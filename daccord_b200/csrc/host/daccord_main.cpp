@@ -1,4 +1,4 @@
-// daccord_main.cpp -- `daccord [options] reads.las reads.db` : drop-in command line for the window-consensus path
+// daccord_main.cpp -- `daccord [options] reads.las reads.db [reads2.db]` : drop-in command line for the window-consensus path
 // of gt1/daccord (reference src/daccord.cpp:185-241 help text, :1061-1305 option handling, :2107-2540 main loop),
 // with the per-window consensus running on an H100 through the C ABI in include/daccord_b200.h.
 // Host side (this file + pile.hpp / vote.hpp): LAS + Dazzler-DB input, overlap selection, trace reconstruction,
@@ -32,13 +32,15 @@
 using namespace dhost;
 
 static const char* HELP =
-    "usage: daccord [options] reads.las reads.db\n"
+    "usage: daccord [options] reads.las reads.db [reads2.db]\n"
+    "\treads2.db: B-reads of an asymmetric alignment (daligner reads.db reads2.db); default reads.db\n"
     "\t-t: number of host threads (default: all)\n\t-w: window size (default 40)\n\t-a: advance size (default 10)\n"
     "\t-d: max depth (default unlimited)\n\t-f: produce full sequences\n\t-V: verbosity\n\t-I: read interval i,j (inclusive)\n"
     "\t-J: reads part i,j\n\t-E: error profile file name (default input.las.eprof)\n\t--eprofonly: compute error profile only\n\t--keepeprof: keep an error profile older than the .las (default 1)\n\t-m: minimum window coverage (default 3)\n"
     "\t-e: maximum window error (default unlimited)\n\t-l: minimum length of output (default 0)\n"
     "\t--minfilterfreq: minimum k-mer filter frequency (default 0)\n\t--maxfilterfreq: maximum k-mer filter frequency (default 2)\n"
-    "\t-D: maximum number of alignments considered per read (default 5000)\n\t-k: kmer size lo[,hi] (default 8)\n"
+    "\t-D: maximum number of alignments considered per read (default 5000)\n"
+    "\t--vard: alignments considered per read proportional to its length, max(2v, 2v*length/average length) (default 0 = off, -D applies)\n\t-k: kmer size lo[,hi] (default 8)\n"
     "\t--device: CUDA device ordinal (default 0)\n\t--batchreads: A-reads per GPU batch (default 1024)\n\t--inflight: batches in flight on the GPU (default 3)\n";
 
 struct Args { std::map<std::string, std::string> opt; std::vector<std::string> pos; };
@@ -68,10 +70,12 @@ int main(int argc, char** argv) {
   if (!parse_args(argc, argv, A)) return EXIT_FAILURE;
   if (A.opt.count("h") || A.opt.count("help") || A.pos.size() < 2) { fprintf(stderr, "%s", HELP); return A.pos.size() < 2 && !A.opt.count("h") && !A.opt.count("help") ? EXIT_FAILURE : EXIT_SUCCESS; }
   auto getu = [&](const char* k, uint64_t def) -> uint64_t { auto it = A.opt.find(k); return (it == A.opt.end() || it->second.empty()) ? def : strtoull(it->second.c_str(), nullptr, 10); };
-  const std::string lasfn = A.pos[0], dbfn = A.pos[1];
-  if (A.pos.size() > 2 && A.pos[2] != dbfn) { fprintf(stderr, "[E] asymmetric (DB1 != DB2) input is not supported by this build\n"); return EXIT_FAILURE; }
+  // reads.las reads.db [reads2.db]: A-reads from reads.db, B-reads from reads2.db (reference src/daccord.cpp:2598-2622, :1337-1369)
+  const std::string lasfn = A.pos[0], dbfn = A.pos[1], db2fn = A.pos.size() > 2 ? A.pos[2] : dbfn;
+  const bool asym = db2fn != dbfn;
   if (A.opt.count("deepprofileonly")) { fprintf(stderr, "[E] --deepprofileonly is not supported by this build\n"); return EXIT_FAILURE; }
-  if (getu("vard", 0)) { fprintf(stderr, "[E] --vard is not supported by this build\n"); return EXIT_FAILURE; }
+  const uint64_t vard = getu("vard", 0);                                 // replaces -D when set (src/daccord.cpp:2121-2126)
+  if (vard && asym) { fprintf(stderr, "[E] --vard is not supported for asymmetric (DB1 != DB2) alignments\n"); return EXIT_FAILURE; }     // :1340-1348
   dcu_params prm; memset(&prm, 0, sizeof(prm));
   prm.w = (uint32_t)getu("w", 40); const uint32_t advance = (uint32_t)getu("a", 10);
   prm.k_lo = prm.k_hi = 8;
@@ -90,13 +94,16 @@ int main(int argc, char** argv) {
   auto t_start = std::chrono::steady_clock::now();
   auto lap = [&](const char* what) { fprintf(stderr, "[T] %.3fs %s\n", std::chrono::duration<double>(std::chrono::steady_clock::now() - t_start).count(), what); };
   try {
-    PackedDB db; LasData las;
+    PackedDB db, db2; LasData las;
     fprintf(stderr, "[V] loading %s ...", dbfn.c_str()); read_dazzdb(dbfn, db); fprintf(stderr, "done.\n");
+    if (asym) { fprintf(stderr, "[V] loading %s ...", db2fn.c_str()); read_dazzdb(db2fn, db2); fprintf(stderr, "done.\n"); }
+    const uint64_t nA = db.rlen.size();                                  // A-reads, -I / -J and the output count in reads.db
+    const uint64_t avglen = vard ? average_read_length(db.rlen) : 0;     // --vard only (symmetric: reads.db is also the B database)
     // LAS: index of record offsets per A-read (cached as <las>.dcuidx; reference src/daccord.cpp:1075-1104), then only the shard's byte range
     LasIndex lidx; bool built = false;
     fprintf(stderr, "[V] indexing %s ...", lasfn.c_str()); get_las_index(lasfn, lidx, &built); fprintf(stderr, "%s.\n", built ? "done" : "cached");
     // read range: -J i,j or -I i,j (inclusive) (reference src/daccord.cpp:1116-1227; SURVEY D10)
-    int64_t minaread = 0, maxaread = (int64_t)db.rlen.size() - 1;
+    int64_t minaread = 0, maxaread = (int64_t)nA - 1;
     if (lidx.maxaread >= lidx.minaread) { minaread = lidx.minaread; maxaread = lidx.maxaread; } else maxaread = -1;
     if (A.opt.count("J")) {
       int64_t Icnt, Idiv; if (!parse_pair(A.opt["J"], Icnt, Idiv)) { fprintf(stderr, "[E] unable to parse %s\n", A.opt["J"].c_str()); return EXIT_FAILURE; }
@@ -109,7 +116,12 @@ int main(int argc, char** argv) {
     }
     const int64_t toparead = maxaread >= 0 ? maxaread + 1 : maxaread;
     fprintf(stderr, "[V] minaread=%ld toparead=%ld\n", (long)minaread, (long)toparead);
-    fprintf(stderr, "[V] loading %s ...", lasfn.c_str()); read_las_range(lasfn, lidx, minaread, toparead, las, nthreads); las.build_index(db.rlen.size()); validate_las(las, db.rlen);
+    fprintf(stderr, "[V] loading %s ...", lasfn.c_str()); read_las_range(lasfn, lidx, minaread, toparead, las, nthreads); las.build_index(nA);
+    validate_las(las, db.rlen, asym ? &db2.rlen : nullptr);
+    if (asym) {       // one read space: reads2.db's reads follow reads.db's, so bread moves up by nA (LAS order, and so C6, unchanged)
+      for (auto& o : las.ovl) o.bread += (int32_t)nA;
+      append_dazzdb(db, db2, dbfn, db2fn); db2 = PackedDB();
+    }
     fprintf(stderr, "done (%zu of %ld overlaps).\n", las.ovl.size(), (long)lidx.novl);
     lap("inputs loaded");
     fprintf(stderr, "[V] minfilterfreq=%d maxfilterfreq=%d\n", prm.min_ff, prm.max_ff);
@@ -119,7 +131,7 @@ int main(int argc, char** argv) {
     const bool keepeprof = getu("keepeprof", 1) != 0;
     uint64_t ecnt[4] = {0, 0, 0, 0};
     if (eprof_is_stale(eproffn, lasfn, keepeprof)) {
-      ProfileCounts PC = estimate_profile(db, las, minaread, toparead, maxalign, maxinput, nthreads);
+      ProfileCounts PC = estimate_profile(db, las, minaread, toparead, maxalign, maxinput, nthreads, vard, avglen);
       fprintf(stderr, "usable=%lu unusable=%lu eavg=%g edif=%g\n", (unsigned long)PC.usable, (unsigned long)PC.unusable, PC.eavg, PC.edif);
       write_eprof(eproffn, PC.cnt, PC.eavg, PC.edif);
     }
@@ -158,7 +170,7 @@ int main(int argc, char** argv) {
       }
     }
     lap("contexts ready");
-    PileParams PP; PP.w = prm.w; PP.a = advance; PP.maxalign = maxalign_eff; PP.maxinput = maxinput;
+    PileParams PP; PP.w = prm.w; PP.a = advance; PP.maxalign = maxalign_eff; PP.maxinput = maxinput; PP.vard = vard; PP.avglen = avglen;
     VoteParams VP; VP.producefull = producefull; VP.minlen = minlen;
     uint64_t wellcounter = 0, totwin = 0, totok = 0, totlost = 0;
     std::mutex mu; std::condition_variable cv; int64_t turn = 0; std::atomic<int64_t> next{0}; std::atomic<bool> failed{false}; std::string failmsg;
@@ -180,7 +192,7 @@ int main(int argc, char** argv) {
         if (gpu_pile) {
           std::vector<std::vector<uint32_t>> sels(nr);
 #pragma omp parallel for schedule(dynamic, 8) num_threads(wthreads)
-          for (int64_t r = 0; r < nr; ++r) select_overlaps(las, (uint64_t)(b0 + r), maxinput, sels[r]);
+          for (int64_t r = 0; r < nr; ++r) select_overlaps(las, (uint64_t)(b0 + r), read_limit(db.rlen[b0 + r], maxinput, vard, avglen), sels[r]);
           size_t tot = 0; for (auto& v : sels) tot += v.size();
           std::vector<dcu_overlap> ov; ov.reserve(tot);
           for (auto& sel : sels)

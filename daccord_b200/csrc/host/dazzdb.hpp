@@ -84,5 +84,25 @@ inline void read_dazzdb(const std::string& dbfn, PackedDB& db) {
   if (trim && (int64_t)db.rlen.size() != (int64_t)h.treads)
     throw std::runtime_error("trimmed view holds " + std::to_string(db.rlen.size()) + " reads, header says " + std::to_string(h.treads) + " (cutoff / best flags not understood)");
 }
+// one read space for an asymmetric run (`daccord reads.las A.db B.db`): B's reads are appended to A's as reads nA..nA+nB-1,
+// their byte offsets shifted past A's packed bytes.  The window kernel, the piler and the vote address reads only through
+// boff / rlen, so the combined arena feeds them unchanged; a .las bread then needs nA added.  Slice positions are 32-bit
+// base indices, so the two databases together must stay below 2^32 bases (4 per byte), like a single one.
+inline void append_dazzdb(PackedDB& a, const PackedDB& b, const std::string& afn, const std::string& bfn) {
+  const uint64_t abytes = a.bytes.size() >= 16 ? a.bytes.size() - 16 : 0;          // drop A's 16 padding bytes, keep B's
+  if (abytes + b.bytes.size() >= (1ull << 30))
+    throw std::runtime_error("database larger than 2^32 bases: " + afn + " and " + bfn + " together hold " + std::to_string(abytes + b.bytes.size()) +
+                             " bytes of packed bases (at most " + std::to_string((1ull << 30) - 1) + ")");
+  a.bytes.resize(abytes);
+  a.bytes.insert(a.bytes.end(), b.bytes.begin(), b.bytes.end());
+  for (size_t i = 0; i < b.rlen.size(); ++i) { a.boff.push_back(b.boff[i] + abytes); a.rlen.push_back(b.rlen[i]); }
+}
+// the average read length `--vard` scales by (libmaus2 DatabaseFile::getAverageReadLength, not available here; INTEGRATION.md §3):
+// the integer quotient of the summed length of the reads in the trimmed view by their number, unverified against libmaus2
+inline uint64_t average_read_length(const std::vector<uint32_t>& rlen) {
+  uint64_t s = 0;
+  for (auto l : rlen) s += l;
+  return rlen.empty() ? 0 : s / rlen.size();
+}
 
 }  // namespace dhost

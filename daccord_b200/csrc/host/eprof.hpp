@@ -238,12 +238,12 @@ inline void select_overlaps_profile(const LasData& L, uint64_t aread, uint64_t m
 class ProfileEstimator {
  public:
   enum { EW = 40, EA = 5 };                   // src/daccord.cpp:1279-1280
-  ProfileEstimator(const PackedDB& rdb, const LasData& rL, uint64_t rmaxalign, uint64_t rmaxinput)
-      : db(rdb), L(rL), maxalign(rmaxalign), maxinput(rmaxinput), RP(rdb, rL, PileParams()) {}
+  ProfileEstimator(const PackedDB& rdb, const LasData& rL, uint64_t rmaxalign, uint64_t rmaxinput, uint64_t rvard = 0, uint64_t ravglen = 0)
+      : db(rdb), L(rL), maxalign(rmaxalign), maxinput(rmaxinput), vard(rvard), avglen(ravglen), RP(rdb, rL, PileParams()) {}
 
   // one A-read: adds to C, returns the mean error rate of its consensus windows (0 if none)
   double read(uint64_t aread, ProfileCounts& C) {
-    select_overlaps_profile(L, aread, maxinput, sel);
+    select_overlaps_profile(L, aread, read_limit(db.rlen[aread], maxinput, vard, avglen), sel);
     const size_t nintv = sel.size();
     if (!nintv) return 0.0;
     decode_read(db, (uint32_t)aread, false, RP.abuf);
@@ -298,7 +298,7 @@ class ProfileEstimator {
   }
 
  private:
-  const PackedDB& db; const LasData& L; uint64_t maxalign, maxinput;
+  const PackedDB& db; const LasData& L; uint64_t maxalign, maxinput, vard, avglen;
   ReadPiler RP;                                // for its tile aligner and trace reconstruction
   TrivialConsensus TC;
   std::vector<uint32_t> sel, tmp;
@@ -306,14 +306,16 @@ class ProfileEstimator {
   std::vector<Seq> pile; std::vector<uint8_t> cons;
 };
 
-// A-reads [lo, min(hi, lo + 1024)); per-read results are combined in read order whatever the thread count
-inline ProfileCounts estimate_profile(const PackedDB& db, const LasData& L, int64_t lo, int64_t hi, uint64_t maxalign, uint64_t maxinput, int nthreads) {
+// A-reads [lo, min(hi, lo + 1024)); per-read results are combined in read order whatever the thread count.  vard / avglen: --vard
+// and the DB's average read length (read_limit in pile.hpp; the estimator applies the same per-read limit, src/daccord.cpp:1689-1694)
+inline ProfileCounts estimate_profile(const PackedDB& db, const LasData& L, int64_t lo, int64_t hi, uint64_t maxalign, uint64_t maxinput, int nthreads,
+                                      uint64_t vard = 0, uint64_t avglen = 0) {
   const int64_t top = std::min(hi, lo + 1024), nr = std::max<int64_t>(top - lo, 0);
   std::vector<ProfileCounts> per(nr); std::vector<double> rate(nr, 0.0);
   if (nthreads < 1) nthreads = 1;
 #pragma omp parallel num_threads(nthreads)
   {
-    ProfileEstimator PE(db, L, maxalign, maxinput);
+    ProfileEstimator PE(db, L, maxalign, maxinput, vard, avglen);
 #pragma omp for schedule(dynamic, 1)
     for (int64_t i = 0; i < nr; ++i) {
       if (L.aidx[lo + i] == L.aidx[lo + i + 1]) continue;

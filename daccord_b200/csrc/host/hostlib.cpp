@@ -23,6 +23,8 @@ using namespace dhost;
 
 struct dh_data {
   PackedDB db; LasData las;
+  uint64_t nA = 0;                                               // A-reads: reads [0, nA) of db; a two-DB dataset holds the B database's reads after them
+  bool asym = false;                                             // loaded from two databases (dh_data_load2)
   uint64_t st_match = 0, st_mis = 0, st_ins = 0, st_del = 0;     // error profile counts (reference GAS, src/daccord.cpp:1867-1880)
   Truth truth;                                                   // simulated data only, on request: genome + edit scripts (truth.hpp)
   std::string err;
@@ -36,15 +38,17 @@ struct dh_batch {
 
 extern "C" {
 
-dh_data* dh_sim_create_ex(uint64_t genome_len, uint64_t read_len, double coverage, double p_ins, double p_del, double p_sub, double repeat_frac,
-                          uint64_t seed, int32_t tspace, uint64_t min_ovl, int keep) {
+// read_len_spread: SimParams::read_len_spread (0 = every read read_len genome bases, the data of dh_sim_create_ex)
+dh_data* dh_sim_create_spread(uint64_t genome_len, uint64_t read_len, double coverage, double p_ins, double p_del, double p_sub, double repeat_frac,
+                              uint64_t seed, int32_t tspace, uint64_t min_ovl, int keep, double read_len_spread) {
   try {
     SimParams P; P.genome_len = genome_len; P.read_len = read_len; P.coverage = coverage; P.p_ins = p_ins; P.p_del = p_del; P.p_sub = p_sub;
+    P.read_len_spread = read_len_spread;
     P.repeat_frac = repeat_frac; P.seed_genome = 0xDACC01 ^ (seed * 0x9E3779B97F4A7C15ull); P.seed_sample = 0xDACC02 ^ (seed * 0xC2B2AE3D27D4EB4Full); P.seed_err = 0xDACC03 ^ (seed * 0x165667B19E3779F9ull);
     std::vector<uint8_t> G; make_genome(P, G);
     std::vector<SimRead> reads; make_reads(P, G, reads);
     std::unique_ptr<dh_data> D(new dh_data());
-    pack_reads(reads, D->db);
+    pack_reads(reads, D->db); D->nA = D->db.rlen.size();
     make_overlaps(reads, tspace, min_ovl, D->las);
     for (auto& r : reads) {                 // error profile of the simulation itself (what daccord would estimate, src/daccord.cpp:1652-1865)
       D->st_ins += r.n_ins; D->st_del += r.n_del; D->st_mis += r.n_sub; D->st_match += r.glen - r.n_del - r.n_sub;
@@ -52,6 +56,10 @@ dh_data* dh_sim_create_ex(uint64_t genome_len, uint64_t read_len, double coverag
     if (keep) keep_truth(G, reads, D->truth);
     return D.release();
   } catch (...) { return nullptr; }
+}
+dh_data* dh_sim_create_ex(uint64_t genome_len, uint64_t read_len, double coverage, double p_ins, double p_del, double p_sub, double repeat_frac,
+                          uint64_t seed, int32_t tspace, uint64_t min_ovl, int keep) {
+  return dh_sim_create_spread(genome_len, read_len, coverage, p_ins, p_del, p_sub, repeat_frac, seed, tspace, min_ovl, keep, 0.0);
 }
 dh_data* dh_sim_create(uint64_t genome_len, uint64_t read_len, double coverage, double p_ins, double p_del, double p_sub, double repeat_frac,
                        uint64_t seed, int32_t tspace, uint64_t min_ovl) {
@@ -66,16 +74,30 @@ int dh_truth_eval(dh_data* d, const char* fasta, uint64_t len, uint64_t max_read
   out6[0] = S.segments; out6[1] = S.bases; out6[2] = S.truth_bases; out6[3] = S.edits; out6[4] = S.raw_events; out6[5] = S.reads;
   return 0;
 }
-dh_data* dh_data_load(const char* lasfn, const char* dbfn) {
+// A-reads from dbfn, B-reads from db2fn (null or the same name: symmetric), as `daccord lasfn dbfn db2fn` reads them: one read space,
+// db2fn's reads numbered after dbfn's (append_dazzdb) and every bread moved up by their count once the records are checked against both
+dh_data* dh_data_load2(const char* lasfn, const char* dbfn, const char* db2fn) {
   std::unique_ptr<dh_data> D(new dh_data());
-  try { read_dazzdb(dbfn, D->db); read_las(lasfn, D->las); D->las.build_index(D->db.rlen.size()); validate_las(D->las, D->db.rlen); } catch (std::exception& e) { fprintf(stderr, "[E] %s\n", e.what()); return nullptr; }
+  try {
+    read_dazzdb(dbfn, D->db); D->nA = D->db.rlen.size();
+    read_las(lasfn, D->las); D->las.build_index(D->nA);
+    D->asym = db2fn && std::string(db2fn) != dbfn;
+    if (!D->asym) validate_las(D->las, D->db.rlen);
+    else {
+      PackedDB B; read_dazzdb(db2fn, B);
+      validate_las(D->las, D->db.rlen, &B.rlen);
+      for (auto& o : D->las.ovl) o.bread += (int32_t)D->nA;
+      append_dazzdb(D->db, B, dbfn, db2fn);
+    }
+  } catch (std::exception& e) { fprintf(stderr, "[E] %s\n", e.what()); return nullptr; }
   return D.release();
 }
+dh_data* dh_data_load(const char* lasfn, const char* dbfn) { return dh_data_load2(lasfn, dbfn, nullptr); }
 // the overlaps of A-reads [first_read, last_read) only, through the offset index (las_index.hpp); out3 = A-read range of the file and its overlap count
 dh_data* dh_data_load_range(const char* lasfn, const char* dbfn, int64_t first_read, int64_t last_read, int nthreads, int64_t* out3) {
   std::unique_ptr<dh_data> D(new dh_data());
   try {
-    read_dazzdb(dbfn, D->db);
+    read_dazzdb(dbfn, D->db); D->nA = D->db.rlen.size();
     LasIndex I; get_las_index(lasfn, I);
     if (out3) { out3[0] = I.minaread; out3[1] = I.maxaread; out3[2] = I.novl; }
     read_las_range(lasfn, I, first_read, last_read, D->las, nthreads);
@@ -90,7 +112,8 @@ int dh_data_write(dh_data* d, const char* lasfn, const char* dbfn) {
   catch (std::exception& e) { d->err = e.what(); return 1; }
   return 0;
 }
-uint64_t dh_data_nreads(dh_data* d) { return d->db.rlen.size(); }
+uint64_t dh_data_nreads(dh_data* d) { return d->nA; }
+uint64_t dh_data_nall(dh_data* d) { return d->db.rlen.size(); }     // A-reads and, after them, the reads of a second database
 uint64_t dh_data_novl(dh_data* d) { return d->las.ovl.size(); }
 uint64_t dh_data_totlen(dh_data* d) { uint64_t t = 0; for (auto l : d->db.rlen) t += l; return t; }
 const uint8_t* dh_data_packed(dh_data* d, uint64_t* nbytes) { *nbytes = d->db.bytes.size(); return d->db.bytes.data(); }
@@ -101,13 +124,23 @@ const char* dh_data_error(dh_data* d) { return d->err.c_str(); }
 
 // windows + slices of A-reads [first_read, last_read); overlap selection, trace reconstruction and slice
 // extraction run on nthreads host threads (reference: OpenMP over A-reads, src/daccord.cpp:2107-2112)
-dh_batch* dh_pile(dh_data* d, uint64_t first_read, uint64_t last_read, uint32_t w, uint32_t a, uint64_t maxalign, uint64_t maxinput, int nthreads) {
+// --vard needs one database (the reference refuses it for DB1 != DB2, src/daccord.cpp:1340-1348); returns the average read length it scales by
+static bool vard_avglen(dh_data* d, uint64_t vard, uint64_t& avglen) {
+  avglen = 0;
+  if (!vard) return true;
+  if (d->asym) { d->err = "--vard is not supported for asymmetric (DB1 != DB2) alignments"; fprintf(stderr, "[E] %s\n", d->err.c_str()); return false; }
+  avglen = average_read_length(d->db.rlen);
+  return true;
+}
+dh_batch* dh_pile_vard(dh_data* d, uint64_t first_read, uint64_t last_read, uint32_t w, uint32_t a, uint64_t maxalign, uint64_t maxinput, uint64_t vard, int nthreads) {
   std::unique_ptr<dh_batch> B(new dh_batch());
-  if (last_read > d->db.rlen.size()) last_read = d->db.rlen.size();
+  uint64_t avglen;
+  if (!vard_avglen(d, vard, avglen)) return nullptr;
+  if (last_read > d->nA) last_read = d->nA;
   if (first_read > last_read) first_read = last_read;
   B->first_read = first_read; B->last_read = last_read;
   const uint64_t nr = last_read - first_read;
-  PileParams P; P.w = w; P.a = a; P.maxalign = maxalign; P.maxinput = maxinput;
+  PileParams P; P.w = w; P.a = a; P.maxalign = maxalign; P.maxinput = maxinput; P.vard = vard; P.avglen = avglen;
   std::vector<std::vector<dcu_window>> wv(nr); std::vector<std::vector<dcu_slice>> sv(nr);
   std::string err;
   if (nthreads < 1) nthreads = 1;
@@ -138,17 +171,22 @@ dh_batch* dh_pile(dh_data* d, uint64_t first_read, uint64_t last_read, uint32_t 
   }
   return B.release();
 }
+dh_batch* dh_pile(dh_data* d, uint64_t first_read, uint64_t last_read, uint32_t w, uint32_t a, uint64_t maxalign, uint64_t maxinput, int nthreads) {
+  return dh_pile_vard(d, first_read, last_read, w, a, maxalign, maxinput, 0, nthreads);
+}
 void dh_batch_destroy(dh_batch* b) { delete b; }
 
 // the overlaps daccord would hand to HandleContext for A-reads [first,last): top-D selection, ordered by abpos
 // (reference src/daccord.cpp:2112-2288), in the dcu_overlap form of the C ABI.  Buffers are malloc'ed (dh_free).
 struct dh_ovlset { std::vector<dcu_overlap> ovl; };
-dh_ovlset* dh_select_overlaps(dh_data* d, uint64_t first_read, uint64_t last_read, uint64_t maxinput) {
+dh_ovlset* dh_select_overlaps_vard(dh_data* d, uint64_t first_read, uint64_t last_read, uint64_t maxinput, uint64_t vard) {
   std::unique_ptr<dh_ovlset> S(new dh_ovlset());
-  if (last_read > d->db.rlen.size()) last_read = d->db.rlen.size();
+  uint64_t avglen;
+  if (!vard_avglen(d, vard, avglen)) return nullptr;
+  if (last_read > d->nA) last_read = d->nA;
   std::vector<uint32_t> sel;
   for (uint64_t r = first_read; r < last_read; ++r) {
-    select_overlaps(d->las, r, maxinput, sel);
+    select_overlaps(d->las, r, read_limit(d->db.rlen[r], maxinput, vard, avglen), sel);
     for (auto i : sel) {
       const Overlap& o = d->las.ovl[i];
       dcu_overlap x; memset(&x, 0, sizeof(x));
@@ -159,6 +197,7 @@ dh_ovlset* dh_select_overlaps(dh_data* d, uint64_t first_read, uint64_t last_rea
   }
   return S.release();
 }
+dh_ovlset* dh_select_overlaps(dh_data* d, uint64_t first_read, uint64_t last_read, uint64_t maxinput) { return dh_select_overlaps_vard(d, first_read, last_read, maxinput, 0); }
 const dcu_overlap* dh_ovlset_data(dh_ovlset* s, uint64_t* n) { *n = s->ovl.size(); return s->ovl.data(); }
 void dh_ovlset_destroy(dh_ovlset* s) { delete s; }
 const uint16_t* dh_data_trace(dh_data* d, uint64_t* n) { *n = d->las.trace.size(); return d->las.trace.data(); }
@@ -213,16 +252,47 @@ char* dh_vote(dh_data* d, dh_batch* b, const dcu_result* res, const uint8_t* con
 }
 // error profile estimated from the data itself over A-reads [first_read, min(last_read, first_read + 1024)) (reference
 // src/daccord.cpp:1652-1880): out7 = matches, mismatches, insertions, deletions, usable windows, unusable windows, reads; dout2 = eavg, edif
-int dh_estimate_profile(dh_data* d, int64_t first_read, int64_t last_read, uint64_t maxalign, uint64_t maxinput, int nthreads, uint64_t* out7, double* dout2) {
+int dh_estimate_profile_vard(dh_data* d, int64_t first_read, int64_t last_read, uint64_t maxalign, uint64_t maxinput, uint64_t vard, int nthreads, uint64_t* out7, double* dout2) {
   try {
+    uint64_t avglen;
+    if (!vard_avglen(d, vard, avglen)) return 1;
     if (first_read < 0) first_read = 0;
-    if (last_read < 0 || last_read > (int64_t)d->db.rlen.size()) last_read = (int64_t)d->db.rlen.size();
-    ProfileCounts C = estimate_profile(d->db, d->las, first_read, last_read, maxalign, maxinput, nthreads);
+    if (last_read < 0 || last_read > (int64_t)d->nA) last_read = (int64_t)d->nA;
+    ProfileCounts C = estimate_profile(d->db, d->las, first_read, last_read, maxalign, maxinput, nthreads, vard, avglen);
     for (int i = 0; i < 4; ++i) out7[i] = C.cnt[i];
     out7[4] = C.usable; out7[5] = C.unusable; out7[6] = C.reads;
     if (dout2) { dout2[0] = C.eavg; dout2[1] = C.edif; }
     return 0;
   } catch (std::exception& e) { d->err = e.what(); return 1; }
+}
+int dh_estimate_profile(dh_data* d, int64_t first_read, int64_t last_read, uint64_t maxalign, uint64_t maxinput, int nthreads, uint64_t* out7, double* dout2) {
+  return dh_estimate_profile_vard(d, first_read, last_read, maxalign, maxinput, 0, nthreads, out7, dout2);
+}
+// derived data sets (tests of two-DB runs): a Dazzler DB of reads [r0, r1) of this dataset, in order
+int dh_data_write_db_subset(dh_data* d, const char* dbfn, uint64_t r0, uint64_t r1) {
+  try {
+    if (r1 > d->db.rlen.size() || r0 > r1) throw std::runtime_error("read range outside the dataset");
+    PackedDB S; uint64_t tot = 0;
+    for (uint64_t r = r0; r < r1; ++r) { S.boff.push_back(tot); S.rlen.push_back(d->db.rlen[r]); tot += ((uint64_t)d->db.rlen[r] + 3) / 4; }
+    S.bytes.assign(tot + 16, 0);
+    for (uint64_t r = r0; r < r1; ++r) memcpy(S.bytes.data() + S.boff[r - r0], d->db.bytes.data() + d->db.boff[r], ((size_t)d->db.rlen[r] + 3) / 4);
+    write_dazzdb(dbfn, S);
+  } catch (std::exception& e) { d->err = e.what(); return 1; }
+  return 0;
+}
+// ... and a .las of the records with aread in [a0, a1) and bread in [b0, b1), in file order, renumbered aread - ashift, bread - bshift
+int dh_data_write_las_filtered(dh_data* d, const char* lasfn, int64_t a0, int64_t a1, int64_t ashift, int64_t b0, int64_t b1, int64_t bshift) {
+  try {
+    LasData F; F.tspace = d->las.tspace;
+    for (const Overlap& o : d->las.ovl) {
+      if (o.aread < a0 || o.aread >= a1 || o.bread < b0 || o.bread >= b1) continue;
+      Overlap x = o; x.aread = (int32_t)(o.aread - ashift); x.bread = (int32_t)(o.bread - bshift); x.trace_off = F.trace.size();
+      F.trace.insert(F.trace.end(), d->las.trace.begin() + (int64_t)o.trace_off, d->las.trace.begin() + (int64_t)(o.trace_off + (uint64_t)o.tlen));
+      F.ovl.push_back(x);
+    }
+    write_las(lasfn, F);
+  } catch (std::exception& e) { d->err = e.what(); return 1; }
+  return 0;
 }
 // FastA text for the segments of the GPU vote; counter as in dh_vote; malloc'ed result
 char* dh_format_segments(const dcu_segment* seg, uint64_t nseg, const char* chars, uint64_t* counter, uint64_t* outlen) {

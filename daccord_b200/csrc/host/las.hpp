@@ -35,16 +35,18 @@ struct LasData {
 };
 
 // every record must refer to reads of the database and stay inside them: the .las and the .db have to belong together
-// (the reference gets this check from libmaus2's DB accessors; a wrong .db must not become an out-of-bounds access here)
-inline void validate_las(const LasData& L, const std::vector<uint32_t>& rlen) {
-  const int64_t n = (int64_t)rlen.size();
+// (the reference gets this check from libmaus2's DB accessors; a wrong .db must not become an out-of-bounds access here).
+// rlenB: the read lengths of the B database of an asymmetric run (`daccord reads.las A.db B.db`), whose bread counts in B; null = B is A
+inline void validate_las(const LasData& L, const std::vector<uint32_t>& rlen, const std::vector<uint32_t>* rlenB = nullptr) {
+  const std::vector<uint32_t>& rb = rlenB ? *rlenB : rlen;
+  const int64_t n = (int64_t)rlen.size(), nb = (int64_t)rb.size();
   for (size_t i = 0; i < L.ovl.size(); ++i) {
     const Overlap& o = L.ovl[i];
-    const bool ok = o.aread >= 0 && o.aread < n && o.bread >= 0 && o.bread < n && o.abpos >= 0 && o.abpos < o.aepos && (uint32_t)o.aepos <= rlen[o.aread] &&
-                    o.bbpos >= 0 && o.bbpos <= o.bepos && (uint32_t)o.bepos <= rlen[o.bread] && o.tlen >= 0 && (o.tlen & 1) == 0 && o.trace_off + (uint64_t)o.tlen <= L.trace.size();
+    const bool ok = o.aread >= 0 && o.aread < n && o.bread >= 0 && o.bread < nb && o.abpos >= 0 && o.abpos < o.aepos && (uint32_t)o.aepos <= rlen[o.aread] &&
+                    o.bbpos >= 0 && o.bbpos <= o.bepos && (uint32_t)o.bepos <= rb[o.bread] && o.tlen >= 0 && (o.tlen & 1) == 0 && o.trace_off + (uint64_t)o.tlen <= L.trace.size();
     if (!ok) throw std::runtime_error("LAS does not match DB: record " + std::to_string(i) + " (aread " + std::to_string(o.aread) + ", bread " + std::to_string(o.bread) +
                                       ", a [" + std::to_string(o.abpos) + "," + std::to_string(o.aepos) + "), b [" + std::to_string(o.bbpos) + "," + std::to_string(o.bepos) + ")) of " +
-                                      std::to_string(n) + " reads");
+                                      std::to_string(n) + " reads" + (rlenB ? " (B: " + std::to_string(nb) + " reads)" : std::string()));
   }
 }
 

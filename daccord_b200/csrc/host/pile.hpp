@@ -22,7 +22,17 @@ struct PileParams {
   uint32_t w = 40, a = 10;
   uint64_t maxalign = std::numeric_limits<uint64_t>::max();   // -d
   uint64_t maxinput = 5000;                                    // -D
+  uint64_t vard = 0, avglen = 0;                               // --vard and the DB's average read length (read_limit)
 };
+
+// overlaps considered for an A-read of length rl: -D, or with --vard v a limit proportional to the read's length,
+// max(2v, 1, round(2v rl / avglen)) (reference src/daccord.cpp:2121-2126, :1689-1694; avglen: average_read_length in dazzdb.hpp)
+inline uint64_t read_limit(uint64_t rl, uint64_t maxinput, uint64_t vard, uint64_t avglen) {
+  if (!vard) return maxinput;
+  const uint64_t lo = std::max<uint64_t>(2 * vard, 1);
+  if (!avglen) return lo;                                      // no bases in the DB: only empty reads, nothing to scale
+  return std::max(lo, (uint64_t)(2.0 * (double)vard * (double)rl / (double)avglen + 0.5));
+}
 
 // reference HandleContext::Windows (src/HandleContext.hpp:382-447)
 struct WindowsOf {
@@ -86,7 +96,7 @@ struct ReadPiler {
 
   // appends the windows of A-read `aread` (and their slices) to win / sl; returns number of windows
   uint64_t pile(uint64_t aread, std::vector<dcu_window>& win, std::vector<dcu_slice>& sl) {
-    select_overlaps(L, aread, P.maxinput, sel);
+    select_overlaps(L, aread, read_limit(db.rlen[aread], P.maxinput, P.vard, P.avglen), sel);
     const uint64_t nintv = sel.size();
     if (!nintv) return 0;
     decode_read(db, (uint32_t)aread, false, abuf);

@@ -37,6 +37,7 @@ struct SimParams {
   uint64_t genome_len = 100000; uint64_t read_len = 10000; double coverage = 40.0;
   double p_ins = 0.09, p_del = 0.045, p_sub = 0.015;
   double repeat_frac = 0.0;          // fraction of the genome covered by tandem repeats (unit 50-500 bp)
+  double read_len_spread = 0.0;      // > 0: each read's genome length uniform in read_len * [1 - spread, 1 + spread] (0: all read_len, no extra draw)
   uint64_t seed_genome = 0xDACC01, seed_sample = 0xDACC02, seed_err = 0xDACC03;
 };
 
@@ -82,10 +83,13 @@ inline void make_reads(const SimParams& P, const std::vector<uint8_t>& G, std::v
   if (n < 1) n = 1;
   reads.resize(n);
   uint64_t rl = std::min(P.read_len, P.genome_len);
+  const uint64_t rlo = P.read_len_spread > 0 ? std::max<uint64_t>(1, (uint64_t)((double)rl * (1.0 - std::min(P.read_len_spread, 1.0)))) : rl;
+  const uint64_t rhi = P.read_len_spread > 0 ? std::min(P.genome_len, (uint64_t)((double)rl * (1.0 + P.read_len_spread))) : rl;
   for (uint64_t i = 0; i < n; ++i) {
-    uint64_t gstart = (P.genome_len > rl) ? rs.below(P.genome_len - rl + 1) : 0;
+    const uint64_t len = rhi > rlo ? rlo + rs.below(rhi - rlo + 1) : rl;
+    uint64_t gstart = (P.genome_len > len) ? rs.below(P.genome_len - len + 1) : 0;
     bool rc = (rs.next() & 1) != 0;
-    make_read(G, gstart, rl, rc, P, re, reads[i]);
+    make_read(G, gstart, len, rc, P, re, reads[i]);
   }
 }
 

@@ -18,10 +18,10 @@ def lib():
         if not os.path.exists(HOST_LIB_PATH):
             raise DcuError("host library %s not built: run `python -m daccord_b200.build`" % HOST_LIB_PATH)
         L = C.CDLL(HOST_LIB_PATH)
-        for f in ("dh_sim_create", "dh_sim_create_ex", "dh_data_load", "dh_data_load_range", "dh_pile", "dh_vote", "dh_data_packed", "dh_batch_windows", "dh_batch_slices", "dh_batch_read_first",
+        for f in ("dh_sim_create", "dh_sim_create_ex", "dh_sim_create_spread", "dh_data_load", "dh_data_load2", "dh_pile_vard", "dh_select_overlaps_vard", "dh_data_load_range", "dh_pile", "dh_vote", "dh_data_packed", "dh_batch_windows", "dh_batch_slices", "dh_batch_read_first",
                   "dh_select_overlaps", "dh_ovlset_data", "dh_data_trace", "dh_data_boff", "dh_data_rlen", "dh_format_segments"):
             getattr(L, f).restype = C.c_void_p
-        for f in ("dh_data_nreads", "dh_data_novl", "dh_data_totlen"):
+        for f in ("dh_data_nreads", "dh_data_nall", "dh_data_novl", "dh_data_totlen"):
             getattr(L, f).restype = C.c_uint64
         L.dh_data_error.restype = C.c_char_p
         L.dh_data_readlen.restype = C.c_uint32
@@ -38,9 +38,12 @@ class Dataset:
         self.h = C.c_void_p(handle)
 
     @staticmethod
-    def simulate(genome_len, read_len=10000, coverage=40.0, p_ins=0.09, p_del=0.045, p_sub=0.015, repeat_frac=0.0, seed=0, tspace=100, min_ovl=1000, keep_truth=False):
-        return Dataset(lib().dh_sim_create_ex(C.c_uint64(genome_len), C.c_uint64(read_len), C.c_double(coverage), C.c_double(p_ins), C.c_double(p_del),
-                                              C.c_double(p_sub), C.c_double(repeat_frac), C.c_uint64(seed), C.c_int32(tspace), C.c_uint64(min_ovl), C.c_int(int(keep_truth))))
+    def simulate(genome_len, read_len=10000, coverage=40.0, p_ins=0.09, p_del=0.045, p_sub=0.015, repeat_frac=0.0, seed=0, tspace=100, min_ovl=1000, keep_truth=False,
+                 read_len_spread=0.0):
+        """read_len_spread > 0: each read covers a genome length drawn uniformly from read_len * [1 - spread, 1 + spread] (0: all read_len)"""
+        return Dataset(lib().dh_sim_create_spread(C.c_uint64(genome_len), C.c_uint64(read_len), C.c_double(coverage), C.c_double(p_ins), C.c_double(p_del),
+                                                  C.c_double(p_sub), C.c_double(repeat_frac), C.c_uint64(seed), C.c_int32(tspace), C.c_uint64(min_ovl), C.c_int(int(keep_truth)),
+                                                  C.c_double(read_len_spread)))
 
     def truth_eval(self, fasta, max_read=2**62):
         """corrected FastA (bytes) against the simulated truth (keep_truth=True): dict with the corrected / truth bases compared, their edit distance
@@ -52,8 +55,9 @@ class Dataset:
         return {"segments": seg, "reads": nr, "corrected_bases": b, "truth_bases": tb, "edit_distance": ed, "erate": ed / max(tb, 1), "raw_error_events": raw, "raw_erate": raw / max(tb, 1)}
 
     @staticmethod
-    def load(las, db):
-        return Dataset(lib().dh_data_load(las.encode(), db.encode()))
+    def load(las, db, db2=None):
+        """db2: the B-read database of an asymmetric .las (`daccord las db db2`); its reads are numbered after db's, as reads nreads..nall-1"""
+        return Dataset(lib().dh_data_load2(las.encode(), db.encode(), None if db2 is None else db2.encode()))
 
     @staticmethod
     def load_range(las, db, first, last, nthreads=0):
@@ -67,6 +71,17 @@ class Dataset:
         if lib().dh_data_write(self.h, las.encode(), db.encode()):
             raise DcuError(lib().dh_data_error(self.h).decode())
 
+    def write_db_subset(self, db, first, last):
+        """a Dazzler DB of reads [first, last) of this dataset"""
+        if lib().dh_data_write_db_subset(self.h, db.encode(), C.c_uint64(first), C.c_uint64(last)):
+            raise DcuError(lib().dh_data_error(self.h).decode())
+
+    def write_las_filtered(self, las, a_range, b_range, a_shift=0, b_shift=0):
+        """a .las of the records with aread in [a_range) and bread in [b_range), in file order, renumbered aread - a_shift, bread - b_shift"""
+        if lib().dh_data_write_las_filtered(self.h, las.encode(), C.c_int64(a_range[0]), C.c_int64(a_range[1]), C.c_int64(a_shift),
+                                            C.c_int64(b_range[0]), C.c_int64(b_range[1]), C.c_int64(b_shift)):
+            raise DcuError(lib().dh_data_error(self.h).decode())
+
     def close(self):
         if self.h:
             lib().dh_data_destroy(self.h)
@@ -74,7 +89,13 @@ class Dataset:
 
     @property
     def nreads(self):
+        """A-reads (the first database)"""
         return lib().dh_data_nreads(self.h)
+
+    @property
+    def nall(self):
+        """all reads of the packed database: the A-reads, then those of a second database (Dataset.load with db2)"""
+        return lib().dh_data_nall(self.h)
 
     @property
     def novl(self):
@@ -97,30 +118,33 @@ class Dataset:
         ln = m + mis + dele
         return ins / ln, dele / ln, 1.0 - (mis + dele + ins) / ln
 
-    def estimate_profile(self, first=0, last=None, maxalign=2**64 - 1, maxinput=5000, nthreads=0):
+    def estimate_profile(self, first=0, last=None, maxalign=2**64 - 1, maxinput=5000, nthreads=0, vard=0):
         """error profile estimated from the overlaps themselves (reference src/daccord.cpp:1652-1880): dict with the four step counts,
         usable / unusable window counts, reads visited and (eavg, edif)"""
         a = (C.c_uint64 * 7)()
         d = (C.c_double * 2)()
         last = -1 if last is None else last
-        if lib().dh_estimate_profile(self.h, C.c_int64(first), C.c_int64(last), C.c_uint64(maxalign), C.c_uint64(maxinput), C.c_int(nthreads or (os.cpu_count() or 1)), a, d):
+        if lib().dh_estimate_profile_vard(self.h, C.c_int64(first), C.c_int64(last), C.c_uint64(maxalign), C.c_uint64(maxinput), C.c_uint64(vard),
+                                          C.c_int(nthreads or (os.cpu_count() or 1)), a, d):
             raise DcuError(lib().dh_data_error(self.h).decode())
         keys = ("matches", "mismatches", "insertions", "deletions", "usable", "unusable", "reads")
         out = {k: int(v) for k, v in zip(keys, a)}
         out["eavg"], out["edif"] = float(d[0]), float(d[1])
         return out
 
-    def overlaps(self, first=0, last=None, maxinput=5000):
-        """selected overlaps of A-reads [first,last) in dcu_overlap form + the trace array + read offsets / lengths (numpy copies)"""
+    def overlaps(self, first=0, last=None, maxinput=5000, vard=0):
+        """selected overlaps of A-reads [first,last) in dcu_overlap form + the trace array + read offsets / lengths of all reads (numpy copies)"""
         last = self.nreads if last is None else last
-        h = lib().dh_select_overlaps(self.h, C.c_uint64(first), C.c_uint64(last), C.c_uint64(maxinput))
+        h = lib().dh_select_overlaps_vard(self.h, C.c_uint64(first), C.c_uint64(last), C.c_uint64(maxinput), C.c_uint64(vard))
+        if not h:
+            raise DcuError(lib().dh_data_error(self.h).decode())
         n = C.c_uint64(0)
         p = lib().dh_ovlset_data(C.c_void_p(h), C.byref(n))
         ovl = np.frombuffer((C.c_uint8 * (n.value * 48)).from_address(p), dtype=OVERLAP_DT).copy() if n.value else np.zeros(0, OVERLAP_DT)
         lib().dh_ovlset_destroy(C.c_void_p(h))
         p = lib().dh_data_trace(self.h, C.byref(n))
         trace = np.frombuffer((C.c_uint8 * (n.value * 2)).from_address(p), dtype=np.uint16).copy() if n.value else np.zeros(0, np.uint16)
-        nr = self.nreads
+        nr = self.nall
         boff = np.frombuffer((C.c_uint8 * (nr * 8)).from_address(lib().dh_data_boff(self.h)), dtype=np.uint64).copy()
         rlen = np.frombuffer((C.c_uint8 * (nr * 4)).from_address(lib().dh_data_rlen(self.h)), dtype=np.uint32).copy()
         return ovl, trace, boff, rlen
@@ -129,10 +153,11 @@ class Dataset:
     def tspace(self):
         return int(lib().dh_data_tspace(self.h))
 
-    def pile(self, first=0, last=None, w=40, a=10, maxalign=2**64 - 1, maxinput=5000, nthreads=0):
+    def pile(self, first=0, last=None, w=40, a=10, maxalign=2**64 - 1, maxinput=5000, nthreads=0, vard=0):
         last = self.nreads if last is None else last
         nthreads = nthreads or (os.cpu_count() or 1)
-        b = lib().dh_pile(self.h, C.c_uint64(first), C.c_uint64(last), C.c_uint32(w), C.c_uint32(a), C.c_uint64(maxalign), C.c_uint64(maxinput), C.c_int(nthreads))
+        b = lib().dh_pile_vard(self.h, C.c_uint64(first), C.c_uint64(last), C.c_uint32(w), C.c_uint32(a), C.c_uint64(maxalign), C.c_uint64(maxinput),
+                               C.c_uint64(vard), C.c_int(nthreads))
         if not b:
             raise DcuError("piling failed")
         return Batch(self, b)

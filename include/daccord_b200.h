@@ -76,7 +76,9 @@ typedef struct dcu_ctx dcu_ctx;
 int dcu_create(const dcu_params* params, int device, dcu_ctx** out);
 void dcu_destroy(dcu_ctx* ctx);
 /* packed 2-bit read database, Dazzler .bps layout: 4 bases per byte, first base in the top
- * two bits (replaces DecodedReadContainer, reference src/DecodedReadContainer.hpp:81-84) */
+ * two bits (replaces DecodedReadContainer, reference src/DecodedReadContainer.hpp:81-84).
+ * Two databases (an asymmetric .las, `daligner A.db B.db`): pass A's bytes followed by B's; to dcu_pile / dcu_vote pass the
+ * concatenated offset tables (B's shifted by A's byte count) and length tables, and overlaps whose bread has A's read count added. */
 int dcu_set_reads(dcu_ctx* ctx, const uint8_t* packed, uint64_t nbytes);
 /* same, but the buffer is already resident in device memory on ctx's device (e.g. after an
  * ncclBroadcast of the database); the library does not take ownership */
@@ -96,7 +98,8 @@ int dcu_download(dcu_ctx* ctx, dcu_result* res, uint8_t* cons, uint8_t* ops);
  * (OverlapDataInterface::computeTrace per activated overlap, advanceA / getStringLengthUsed per window, the active set
  * ordered by (escore<<32)|z).  Input: the overlaps the caller selected for its A-reads (reference
  * src/daccord.cpp:2112-2288: top -D by score, ordered by abpos), grouped by A-read in ascending order, with their
- * trace points.  The descriptors are built in device memory and become the resident batch (as after dcu_upload). */
+ * trace points.  The descriptors are built in device memory and become the resident batch (as after dcu_upload).
+ * read_boff / read_len cover every read an overlap names: with two databases, the combined read space of dcu_set_reads. */
 typedef struct dcu_overlap {
   int32_t abpos, aepos, bbpos, bepos; uint32_t flags; int32_t aread, bread, diffs;
   int32_t tlen, reserved;       /* number of trace values (2 per tile) */
