@@ -88,6 +88,11 @@ class Engine:
         except Exception:
             pass
 
+    def set_max_depth(self, max_slices):
+        """deepest window (slices, A included) that gets a consensus, 1..65535, default 2047; above 2047 a wide pass runs what the
+        16-bit passes cannot hold (dcu_set_max_depth).  Call before upload / pile / run."""
+        self._ck(self.lib.dcu_set_max_depth(self.ctx, C.c_uint32(max_slices)))
+
     def set_reads(self, packed):
         packed = np.ascontiguousarray(packed, np.uint8)
         self._ck(self.lib.dcu_set_reads(self.ctx, _p(packed), C.c_uint64(packed.size)))
@@ -151,6 +156,12 @@ class Engine:
         c, d = C.c_uint64(0), C.c_uint64(0); e, f = C.c_uint32(0), C.c_uint32(0)
         self._ck(self.lib.dcu_last_stats2(self.ctx, C.byref(c), C.byref(d), C.byref(e), C.byref(f)))
         return {"launches": a.value, "hard_windows": b.value, "second_pass_windows": c.value, "lost_windows": d.value, "smem_warps": e.value, "smem_bytes_per_warp": f.value}
+
+    def wide_stats(self):
+        """the wide pass of the last launch: windows it ran, its warps, bytes of slab (dcu_last_wide_stats)"""
+        a, b, c = C.c_uint64(0), C.c_uint32(0), C.c_uint64(0)
+        self._ck(self.lib.dcu_last_wide_stats(self.ctx, C.byref(a), C.byref(b), C.byref(c)))
+        return {"wide_windows": a.value, "wide_warps": b.value, "wide_slab_bytes": c.value}
 
     def tables(self, which):
         """the tables the kernel reads, copied back from the device (see dcu_get_tables)"""

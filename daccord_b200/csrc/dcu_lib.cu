@@ -2,7 +2,8 @@
 // One persistent launch per batch: every warp pulls window indices from a global ticket counter and runs
 // dcu::process_window (window_core.cuh) on its private workspace slab.  Windows whose graph does not fit
 // the small (tier 0) slab are queued and re-run by a second launch on large (tier 1) slabs -- still on the
-// GPU; there is no CPU path in this library.
+// GPU; there is no CPU path in this library.  With a raised depth limit (dcu_set_max_depth) what still overflows
+// goes to a third launch of the wide build (namespace dcuw: 32-bit slice offsets and counts).
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstring>
@@ -11,6 +12,8 @@
 #include <algorithm>
 #include <new>
 #include <mutex>
+#include <map>
+#include <tuple>
 #include <chrono>
 #include "window_core.cuh"            // namespace dcu : every workspace field in the warp's HBM slab (overflow passes, deep piles)
 #define DCU_NS dcus
@@ -19,6 +22,9 @@
 #define DCU_NS dcuh
 #define DCU_TIER_SMEM 2
 #include "window_core.cuh"            // namespace dcuh: only the k-mer table in shared memory, at full occupancy (first pass of deep, clean piles)
+#define DCU_NS dcuw
+#define DCU_WIDE 1
+#include "window_core.cuh"            // namespace dcuw: HBM workspace with 32-bit slice offsets and counts (windows beyond 65 000 bases, raised depth limit)
 #include "host_tables.hpp"
 #include "host_caps.hpp"
 #include "pile_host.hpp"
@@ -33,6 +39,10 @@ namespace {
 constexpr int WPB = 16;                // warps per block of the HBM passes
 constexpr int BPS = 2;                 // resident blocks per SM the HBM kernel is compiled for (64 registers / thread)
 constexpr int SWPB = 16;               // most warps per block of the shared-memory pass (one block per SM, 128 registers / thread)
+constexpr int WWPB = 4;                // warps per block of the wide pass (few windows, large slabs: small blocks keep the grid close to the window count)
+constexpr uint32_t DEFAULT_MAX_SLICES = 2047;       // deepest window of a context without dcu_set_max_depth
+constexpr size_t WIDE_BUDGET = 2ull << 30;          // bytes of wide-pass slabs one context allocates at most (three contexts per device: 6 GB of 80)
+constexpr int WIDE_MAX_BASES = 4 << 20;             // bases of the largest window the wide pass takes (a slab of ~140 MB)
 
 struct KArgs {
   const uint8_t* packed; const dcu::Slice* sl; const dcu::Window* win;
@@ -155,6 +165,44 @@ __global__ void __launch_bounds__(WPB * 32, BPS) dcuh_window_kernel(const __grid
     const bool idle = st.ph == dcuh::PH_END;
     bool alldone;
     DCU_STAGE_LOOP(dcuh, (void)0)
+  }
+}
+
+// ---- wide build: as dcu_window_kernel with 32-bit slice offsets and counts, always free running (the windows are few and uneven)
+__global__ void __launch_bounds__(WWPB * 32) dcuw_window_kernel(const __grid_constant__ KArgs a) {
+  extern __shared__ unsigned long long s_vs[];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (a.vs_words) { for (uint32_t i = threadIdx.x; i < a.vs_words; i += blockDim.x) s_vs[i] = dcuw::c_T.VSq[i]; __syncthreads(); }
+  dcuw::Ctx c;
+  c.ws.base = a.slabs + ((size_t)blockIdx.x * (blockDim.x >> 5) + warp) * (size_t)dcuw::c_layout.bytes;
+  c.vsq = a.vs_words ? s_vs : dcuw::c_T.VSq; c.vs_sm = a.vs_words ? 1 : 0; c.epoch = (unsigned long long)a.launch_seq << 32;
+  c.packed = a.packed; c.sl = a.sl;
+  __shared__ int s_done[2][WWPB];
+  const int G = 1, gfirst = 0;
+  auto gsync = [&]() {};
+  const int smask = 0;
+  dcuw::WinState st; st.ph = dcuw::PH_END;
+  uint32_t wi = 0; bool nomore = false; int par = 0;
+  auto publish = [&]() {
+    if (lane == 0) {
+      a.res[wi] = st.res;
+      if (st.res.status == dcuw::ST_OVERFLOW) { unsigned int o = atomicAdd(a.ovf_cnt, 1u); a.ovf_list[o] = wi; }
+    }
+  };
+  for (;; par ^= 1) {
+    while (!nomore && st.ph == dcuw::PH_END) {
+      unsigned int t = 0;
+      if (lane == 0) t = atomicAdd(a.ticket, 1u);
+      t = __shfl_sync(0xffffffffu, t, 0);
+      if (t >= a.n) { nomore = true; break; }
+      wi = a.todo[t];
+      const dcu::Window wd = a.win[wi];
+      dcuw::st_begin(c, st, wd, lane, nullptr);
+      if (st.ph == dcuw::PH_END) publish();
+    }
+    const bool idle = st.ph == dcuw::PH_END;
+    bool alldone;
+    DCU_STAGE_LOOP(dcuw, (void)0)
   }
 }
 
@@ -419,6 +467,10 @@ struct dcu_ctx {
   dcu::Caps capsS{}; dcus::Layout layS{}; int warpsS = 0;   // shared-memory pass: capacities, layout, warps per block
   dcu::Caps capsH{}; dcuh::Layout layH{}; int use_hybrid = 0, hybrid_ok = 0; DevBuf<uint8_t> dslabH; DevBuf<uint32_t> dovfH;   // hybrid pass (k-mer table in shared memory)
   uint64_t nwin = 0, nsl = 0; int maxS = 0, maxB = 0;
+  // wide pass (windows still DCU_WIN_OVERFLOW after tier 1, when dcu_set_max_depth raised the slice limit): slabs allocated per launch
+  uint32_t max_slices = DEFAULT_MAX_SLICES;
+  dcu::Caps capsW{}; dcuw::Layout layW{}; uint8_t* dslabW = nullptr;
+  uint64_t wide = 0; uint32_t wide_warps = 0; uint64_t wide_slab_bytes = 0;
   // piling scratch
   DevBuf<dpile::Ovl> dpo; DevBuf<dpile::ReadInfo> dpr; DevBuf<uint32_t> dprid, dptile, dpbm, dprlen; DevBuf<uint64_t> dpboff; DevBuf<uint16_t> dptrace;
   DevBuf<double> dpmin, dpdiv; DevBuf<unsigned long long> dpact; DevBuf<uint32_t> dpcnt; DevBuf<uint64_t> dpblkw, dpblks;
@@ -537,13 +589,44 @@ int dcu_share_reads(dcu_ctx* ctx, dcu_ctx* owner) {
   return DCU_OK;
 }
 
+int dcu_set_max_depth(dcu_ctx* ctx, uint32_t max_slices) {
+  if (!ctx) return DCU_ERR_PARAM;
+  if (max_slices < 1 || max_slices > 65535) { ctx->err = "max_slices must be 1 .. 65535"; return DCU_ERR_UNSUPPORTED; }
+  CK(cudaSetDevice(ctx->device));
+  const int klimn = (int)std::max<uint32_t>(max_slices, DEFAULT_MAX_SLICES) + 1;      // one column per pile depth; never fewer than the default 2048
+  if (klimn != ctx->HT.KLIMN) {
+    auto& H = ctx->HT;
+    {   // built once per process and parameter set (the contexts of a run all ask for the same table); the lock makes the others wait for it
+      static std::mutex mu; static std::map<std::tuple<double, int, int, int>, std::vector<unsigned long long>> cache;
+      std::lock_guard<std::mutex> g(mu);
+      auto& t = cache[std::make_tuple(ctx->prm.est_cor, (int)ctx->prm.k_lo, (int)ctx->prm.k_hi, klimn)];
+      if (t.empty()) dcu_host::build_klim(ctx->prm.est_cor, (int)ctx->prm.k_lo, (int)ctx->prm.k_hi, klimn, t);
+      H.klim = t;
+    }
+    H.KLIMN = klimn;
+    CK(cudaStreamSynchronize(ctx->stream));        // the old table may still be read by work in flight
+    ctx->dklim.release();
+    CK(ctx->dklim.ensure(H.klim.size()));
+    CK(cudaMemcpy(ctx->dklim.p, H.klim.data(), H.klim.size() * 8, cudaMemcpyHostToDevice));
+    ctx->T.klim = ctx->dklim.p; ctx->T.KLIMN = H.KLIMN;
+  }
+  ctx->max_slices = max_slices;
+  return DCU_OK;
+}
+
 // sizes the workspaces and result buffers for a batch whose descriptors are (or will be) in ctx->dwin / ctx->dsl
 static int finish_batch(dcu_ctx* ctx, int maxS, int maxB, uint64_t totS, uint64_t nwin, uint64_t nsl) {
   if (maxS < 4) maxS = 4;
   if (maxB < 64) maxB = 64;
-  // windows beyond what the 16-bit indices of the kernel address (>= KLIMN slices or > 65000 bases) end as DCU_WIN_OVERFLOW in the
-  // kernel's own capacity checks (load_window); they do not fail the batch
-  if (maxS >= ctx->HT.KLIMN) maxS = ctx->HT.KLIMN - 1;
+  // windows beyond the context's slice limit (2047 unless dcu_set_max_depth raised it) or beyond what the 16-bit offsets of the kernel
+  // address (> 65000 bases) end as DCU_WIN_OVERFLOW in the kernel's own capacity checks (load_window); they do not fail the batch.
+  // With a raised limit, what still overflows after tier 1 goes to the wide pass, whose capacities follow the batch's largest window
+  if ((uint32_t)maxS > ctx->max_slices) maxS = (int)ctx->max_slices;
+  if (ctx->max_slices > DEFAULT_MAX_SLICES) {
+    const int wb = getenv("DCU_WIDE_MAX_BASES") ? atoi(getenv("DCU_WIDE_MAX_BASES")) : WIDE_MAX_BASES;      // test / measurement knob
+    ctx->capsW = dcu_host::make_caps(1, (int)ctx->prm.w, maxS, std::min(maxB, wb > 0 ? wb : WIDE_MAX_BASES));
+    dcuw::make_layout(ctx->capsW, ctx->layW);
+  }
   if (maxB > 65000) maxB = 65000;
   ctx->maxS = maxS; ctx->maxB = maxB;
   // phase-synchronous group size: deep, homogeneous piles gain from large groups (instruction-cache locality); shallow
@@ -812,10 +895,46 @@ static int launch_hybrid(dcu_ctx* ctx, uint32_t n) {
   return DCU_OK;
 }
 
+// wide pass: the n windows in dovf[1] (overflowed in tier 1) on slabs of the wide layout, as many warps as the budget holds (at most one per window);
+// returns the number of windows that overflowed here too (listed in dovf[2]), or all n when no slab can be had -- they keep DCU_WIN_OVERFLOW
+static int launch_wide(dcu_ctx* ctx, uint32_t n, uint32_t* still) {
+  *still = n;
+  const size_t bytes = ctx->layW.bytes;
+  size_t budget = WIDE_BUDGET;
+  { const char* e = getenv("DCU_WIDE_BUDGET_MB"); if (e && atoll(e) > 0) budget = (size_t)atoll(e) << 20; }      // test / measurement knob
+  const size_t warps = std::min<size_t>({(size_t)n, budget / bytes, (size_t)ctx->num_sms * WWPB * 4});
+  if (warps == 0) return DCU_OK;                     // one slab alone is beyond the budget
+  const int wpb = (int)std::min<size_t>(warps, WWPB), grid = (int)(warps / wpb);
+  const size_t total = (size_t)grid * wpb * bytes;
+  if (cudaMalloc((void**)&ctx->dslabW, total) != cudaSuccess) { cudaGetLastError(); ctx->dslabW = nullptr; return DCU_OK; }      // no memory: the windows stay lost
+  ctx->wide_warps = (uint32_t)(grid * wpb); ctx->wide_slab_bytes = total;
+  struct Free { uint8_t*& p; ~Free() { cudaFree(p); p = nullptr; } } free_slabs{ctx->dslabW};      // deep windows are rare: the slabs are not kept between batches
+  CK(cudaMemsetAsync(ctx->dslabW, 0, total, ctx->stream));      // (workspace slabs start zeroed: no slot record carries a tag)
+  CK(cudaMemcpyToSymbolAsync(dcuw::c_layout, &ctx->layW, sizeof(dcuw::Layout), 0, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyToSymbolAsync(dcuw::c_cap, &ctx->capsW, sizeof(dcu::Caps), 0, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyToSymbolAsync(dcuw::c_T, &ctx->T, sizeof(dcu::Tables), 0, cudaMemcpyHostToDevice, ctx->stream));
+  { dcu::Params P = ctx->P; P.defer_ff = 0; ctx->Pl[1] = P; CK(cudaMemcpyToSymbolAsync(dcuw::c_P, &ctx->Pl[1], sizeof(dcu::Params), 0, cudaMemcpyHostToDevice, ctx->stream)); }
+  KArgs a;
+  fill_args(ctx, a, 10, 2, ctx->dovf[1].p, n);
+  a.slabs = ctx->dslabW;
+  size_t vs_bytes = ctx->HT.VSq.size() * sizeof(unsigned long long);
+  if (vs_bytes > 40 * 1024) vs_bytes = 0;
+  a.vs_words = (uint32_t)(vs_bytes / 8);
+  a.sync_group = 1;
+  dcuw_window_kernel<<<grid, wpb * 32, vs_bytes, ctx->stream>>>(a);
+  CK(cudaGetLastError());
+  ctx->launches++;
+  unsigned int cnt[2];
+  CK(cudaMemcpyAsync(cnt, ctx->dcnt.p + 10, sizeof(cnt), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  ctx->wide = n; *still = cnt[1];
+  return DCU_OK;
+}
+
 int dcu_launch(dcu_ctx* ctx, float* kernel_ms) {
   if (!ctx) return DCU_ERR_PARAM;
   CK(cudaSetDevice(ctx->device));
-  ctx->launches = 0; ctx->hard = 0; ctx->second = 0; ctx->lost = 0;
+  ctx->launches = 0; ctx->hard = 0; ctx->second = 0; ctx->lost = 0; ctx->wide = 0; ctx->wide_warps = 0; ctx->wide_slab_bytes = 0;
   if (kernel_ms) *kernel_ms = 0.f;
   if (!ctx->nwin) return DCU_OK;
   std::lock_guard<std::mutex> pass_lock(g_window_pass_lock[ctx->device & 63]);
@@ -849,11 +968,19 @@ int dcu_launch(dcu_ctx* ctx, float* kernel_ms) {
       if (rc) return rc;
       CK(cudaMemcpyAsync(cnt, ctx->dcnt.p + 2, sizeof(cnt), cudaMemcpyDeviceToHost, ctx->stream));
       CK(cudaStreamSynchronize(ctx->stream));
+      const uint32_t* lost_list = ctx->dovf[1].p;
+      if (cnt[1] && ctx->max_slices > DEFAULT_MAX_SLICES) {      // raised depth limit: what is left goes to the wide pass
+        uint32_t still = cnt[1];
+        rc = launch_wide(ctx, cnt[1], &still);
+        if (rc) return rc;
+        if (ctx->wide) lost_list = ctx->dovf[2].p;
+        cnt[1] = still;
+      }
       if (cnt[1]) {
         // beyond every capacity of this build: the windows keep status DCU_WIN_OVERFLOW (the caller treats them like failed windows, as the
         // reference swallows a read's exception, src/daccord.cpp:2466-2478); the batch itself is not an error
         uint32_t wi = 0; dcu::Result r; memset(&r, 0, sizeof(r));
-        CK(cudaMemcpy(&wi, ctx->dovf[1].p, sizeof(wi), cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(&wi, lost_list, sizeof(wi), cudaMemcpyDeviceToHost));
         CK(cudaMemcpy(&r, ctx->dres.p + wi, sizeof(r), cudaMemcpyDeviceToHost));
         char b[192]; snprintf(b, sizeof b, "%u windows exceeded the large-workspace capacities (first: window %u, capacity code %u)", cnt[1], wi, r.err);
         ctx->err = b; ctx->lost = cnt[1];
@@ -966,6 +1093,13 @@ int dcu_last_stats(dcu_ctx* ctx, uint64_t* launches, uint64_t* hard_windows) {
   if (!ctx) return DCU_ERR_PARAM;
   if (launches) *launches = ctx->launches;
   if (hard_windows) *hard_windows = ctx->hard;
+  return DCU_OK;
+}
+int dcu_last_wide_stats(dcu_ctx* ctx, uint64_t* wide_windows, uint32_t* wide_warps, uint64_t* wide_slab_bytes) {
+  if (!ctx) return DCU_ERR_PARAM;
+  if (wide_windows) *wide_windows = ctx->wide;
+  if (wide_warps) *wide_warps = ctx->wide_warps;
+  if (wide_slab_bytes) *wide_slab_bytes = ctx->wide_slab_bytes;
   return DCU_OK;
 }
 int dcu_last_stats2(dcu_ctx* ctx, uint64_t* second_pass_windows, uint64_t* lost_windows, uint32_t* smem_warps, uint32_t* smem_bytes_per_warp) {

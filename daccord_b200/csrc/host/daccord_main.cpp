@@ -147,8 +147,13 @@ int main(int argc, char** argv) {
     // threads (:2107-2112, :2481-2534); here `inflight` worker threads each own a dcu_ctx and walk the batches round robin: while one
     // batch runs the window kernel, the others select overlaps, pile, vote and format (the library serialises only the window passes of
     // the contexts of one device).  Output is released in batch order, sequences numbered like -t1 (SURVEY D6).
-    const uint64_t maxalign_eff = std::min<uint64_t>(maxalign, 2047);       // deeper piles are capped like -d2047 (16-bit slice counts / 2048-entry KmerLimit table)
-    if (maxalign != UINT64_MAX && maxalign > maxalign_eff) fprintf(stderr, "[W] -d%lu capped at %lu\n", (unsigned long)maxalign, (unsigned long)maxalign_eff);
+    // Pile depth in slices (the A window included): -d, the deepest pile -D (or --vard) lets a read of this run have (its overlaps plus the
+    // A window), and the 65 535 slices a window descriptor counts.  Every context computes windows up to that depth (dcu_set_max_depth).
+    uint64_t deepest = maxinput;
+    if (vard) { deepest = 0; for (int64_t r = minaread; r < toparead; ++r) deepest = std::max(deepest, read_limit(db.rlen[r], maxinput, vard, avglen)); }
+    const uint64_t allowed = std::min(maxalign, deepest == UINT64_MAX ? deepest : deepest + 1);
+    const uint64_t maxalign_eff = std::min<uint64_t>(allowed, 65535);
+    if (allowed > maxalign_eff) fprintf(stderr, "[W] windows are capped at %lu slices (-d / -D%s allow %lu)\n", (unsigned long)maxalign_eff, vard ? " / --vard" : "", (unsigned long)allowed);
     const int64_t nbatches = toparead > minaread ? (toparead - minaread + (int64_t)batchreads - 1) / (int64_t)batchreads : 0;
     int inflight = (int)getu("inflight", 3);
     if (inflight < 1) inflight = 1;
@@ -161,6 +166,7 @@ int main(int argc, char** argv) {
       std::vector<std::thread> th;
       for (int i = 0; i < inflight; ++i) th.emplace_back([&, i]() {
         rcs[i] = dcu_create(&prm, device, &ctxs[i]);
+        if (!rcs[i]) rcs[i] = dcu_set_max_depth(ctxs[i], (uint32_t)std::max<uint64_t>(maxalign_eff, 1));
         if (!rcs[i] && i == 0) rcs[i] = dcu_set_reads(ctxs[0], db.bytes.data(), db.bytes.size());
       });
       for (auto& t : th) t.join();

@@ -21,6 +21,8 @@ struct HostTables {
   std::vector<unsigned long long> klim;          // [nk][KLIMN]
 };
 
+inline void build_klim(double est_cor, int k_lo, int k_hi, int klimn, std::vector<unsigned long long>& klim);
+
 // P(read offset = j | true offset = l): (l+1)-fold geometric insertion law convolved with Binomial(l,p_d) deletions
 inline void build_tables(int w, double p_i, double p_d, double est_cor, int k_lo, int k_hi, int klimn, HostTables& T) {
   const int NP = w + 1;
@@ -107,31 +109,39 @@ inline void build_tables(int w, double p_i, double p_d, double est_cor, int k_lo
     while (k < NP && first[k] <= pos) ++k;
     T.suplo[pos] = (uint16_t)j; T.suphi[pos] = (uint16_t)k;
   }
-  // k-mer frequency limits: smallest m with Binomial(n, est_cor^k) CDF >= 0.99 (README convention C3).  The running binomial term
-  // is term * 2^e with term renormalised by frexp after every step: q^n underflows in deep piles (q^n < 2^-1022 from n ~ 770 at
-  // est_cor 0.85, k 3), and a subnormal or zero first term would leave the sum short of 0.99.  Power-of-two scaling is exact, so
-  // wherever the plain double recurrence stays normal the limits are bit for bit the same.
   T.KLIMN = klimn; T.nk = k_hi - k_lo + 1;
-  T.klim.assign((size_t)T.nk * klimn, 0ull);
+  build_klim(est_cor, k_lo, k_hi, klimn, T.klim);
+}
+
+// k-mer frequency limits: smallest m with Binomial(n, est_cor^k) CDF >= 0.99 (README convention C3), [k_hi - k_lo + 1][klimn].  The running
+// binomial term is term * 2^e with term renormalised by frexp after every step: q^n underflows in deep piles (q^n < 2^-1022 from n ~ 770 at
+// est_cor 0.85, k 3), and a subnormal or zero first term would leave the sum short of 0.99.  Power-of-two scaling is exact, so wherever the
+// plain double recurrence stays normal the limits are bit for bit the same.
+// The first term q^n of column n is the first term of column n - 1 times q: it is carried from column to column (the same operations in the
+// same order as n steps from 1.0, so the same bits), which leaves the sum over m as the only per-column cost.  The columns are independent
+// from there and are built in parallel where OpenMP is on.  (klimn = 65 536, est_cor 0.85, k 8: see DESIGN.md section 2 for the time.)
+inline void build_klim(double est_cor, int k_lo, int k_hi, int klimn, std::vector<unsigned long long>& klim) {
+  const int nk = k_hi - k_lo + 1;
+  klim.assign((size_t)nk * klimn, 0ull);
+  std::vector<double> t0(klimn); std::vector<int> e0(klimn);
   for (int kk = k_lo; kk <= k_hi; ++kk) {
-    double pk = std::pow(est_cor, (double)kk);
+    const double pk = std::pow(est_cor, (double)kk);
+    unsigned long long* row = klim.data() + (size_t)(kk - k_lo) * klimn;
+    if (pk == 0.0) continue;                       // every limit 0
+    const double q = 1.0 - pk;
+    if (q == 0.0) { for (int n = 0; n < klimn; ++n) row[n] = (unsigned long long)n; continue; }
+    { double term = 1.0; int e = 0, s; for (int n = 0; n < klimn; ++n) { t0[n] = term; e0[n] = e; term = std::frexp(term * q, &s); e += s; } }
+    const double ratio = pk / q;
+#pragma omp parallel for schedule(dynamic, 64)
     for (int n = 0; n < klimn; ++n) {
       unsigned long long lim = (unsigned long long)n;
-      if (pk == 0.0) lim = 0;
-      else {
-        double q = 1.0 - pk;
-        if (q != 0.0) {
-          double term = 1.0; int e = 0, s;
-          for (int t = 0; t < n; ++t) { term = std::frexp(term * q, &s); e += s; }
-          double ratio = pk / q, sum = 0.0;
-          for (int m = 0; m <= n; ++m) {
-            sum += std::ldexp(term, e);
-            if (sum >= 0.99) { lim = (unsigned long long)m; break; }
-            term = std::frexp(term * (double)(n - m) / (double)(m + 1) * ratio, &s); e += s;
-          }
-        }
+      double term = t0[n], sum = 0.0; int e = e0[n], s;
+      for (int m = 0; m <= n; ++m) {
+        sum += std::ldexp(term, e);
+        if (sum >= 0.99) { lim = (unsigned long long)m; break; }
+        term = std::frexp(term * (double)(n - m) / (double)(m + 1) * ratio, &s); e += s;
       }
-      T.klim[(size_t)(kk - k_lo) * klimn + n] = lim;
+      row[n] = lim;
     }
   }
 }

@@ -29,6 +29,8 @@
 //   DCU_NS = dcus, DCU_TIER_SMEM = 1 : the fields marked S below live in the warp's shared-memory arena, the rest in a (small) slab.
 //   DCU_NS = dcuh, DCU_TIER_SMEM = 2 : only the k-mer table (S = 1: keys, 16-bit values, pre-filter bitmaps, counters) lives in shared memory -- 5 KB
 //                                      per warp, which all 32 resident warps of an SM can have -- everything else in the HBM slab with tier-0 capacities.
+//   DCU_NS = dcuw, DCU_WIDE = 1      : the HBM build with 32-bit per-slice offsets and 32-bit k-mer counts, for windows beyond 65 000 bases
+//                                      (deep piles, up to 65 535 slices): slice offsets and counts are no longer bounded by 16 bits, only by the slab.
 #include "window_types.cuh"
 #ifndef DCU_NS
 #define DCU_NS dcu
@@ -36,10 +38,27 @@
 #ifndef DCU_TIER_SMEM
 #define DCU_TIER_SMEM 0
 #endif
+#ifndef DCU_WIDE
+#define DCU_WIDE 0
+#endif
 
 namespace DCU_NS {
 using namespace dcub;
 using dcub::ballot;                      // (hides the toolkit's global ::ballot)
+
+// per-slice offsets (sw, soff, koff) and k-mer counts (n_freq, n_sfreq and the sort / first / last count lists): 16 bit, except in the wide build.
+// DCU_MAX_BASES: bases of a window beyond which the offsets no longer fit (the wide build checks against the slab's capacity only)
+#if DCU_WIDE
+typedef uint32_t soff_t;
+typedef uint32_t cnt_t;
+#define DCU_OFF_MAX 0xFFFFFFFFu
+#define DCU_MAX_BASES 0x0ffffffe
+#else
+typedef uint16_t soff_t;
+typedef uint16_t cnt_t;
+#define DCU_OFF_MAX 65535u
+#define DCU_MAX_BASES 65000
+#endif
 
 // value of a hash slot and offsets into the instance lists: 16 bit in the shared-memory build (its capacities are small)
 #if DCU_TIER_SMEM
@@ -49,6 +68,9 @@ typedef uint16_t ioff_t;
 #else
 typedef uint32_t ioff_t;                 // hybrid build: instance lists with tier-0 capacities
 #endif
+#elif DCU_WIDE
+typedef unsigned long long hval_t;       // count | node id << 32 (0xFFFF: not a node): counts may pass 2^16
+typedef uint32_t ioff_t;
 #else
 typedef uint32_t hval_t;                 // count | node id << 16 (0xFFFF: not a node)
 typedef uint32_t ioff_t;
@@ -67,17 +89,17 @@ struct Layout { uint32_t off[128]; uint32_t bytes; uint32_t sbytes; };
 // S = 1 (the k-mer table): in the arena of the shared-memory build and of the hybrid build; S = 2: in the arena of the shared-memory build only
 #define DCU_IN_SMEM(S) ((S) == 1 || ((S) == 2 && DCU_TIER_SMEM == 1))
 #define DCU_WS_FIELDS(X)                                                                                              \
-  X(bw, uint32_t, c.BW, 2) X(sw, uint16_t, c.S + 1, 2) X(soff, uint16_t, c.S + 1, 2) X(lenhist, uint16_t, 256, 0)      \
+  X(bw, uint32_t, c.BW, 2) X(sw, soff_t, c.S + 1, 2) X(soff, soff_t, c.S + 1, 2) X(lenhist, uint16_t, 256, 0)          \
   X(hkey, uint32_t, c.H, 1) X(hval, hval_t, c.H, 1) X(hbA, uint32_t, c.NBITS / 32 + 4, 1) X(hbB, uint32_t, c.NBITS / 32 + 4, 1) \
   X(hstate, uint32_t, 4, 1)                                                                                           \
-  X(koff, uint16_t, c.S + 1, 2) X(lastk, uint32_t, c.S, 2)                              \
-  X(ts_k, uint32_t, c.S, 0) X(ts_c, uint16_t, c.S, 0) X(ts_n, uint16_t, c.S, 0)                                        \
-  X(n_kmer, uint32_t, c.NN, 0) X(n_freq, uint16_t, c.NN, 2) X(n_ioff, ioff_t, c.NN, 2)                                 \
+  X(koff, soff_t, c.S + 1, 2) X(lastk, uint32_t, c.S, 2)                                \
+  X(ts_k, uint32_t, c.S, 0) X(ts_c, cnt_t, c.S, 0) X(ts_n, uint16_t, c.S, 0)                                           \
+  X(n_kmer, uint32_t, c.NN, 0) X(n_freq, cnt_t, c.NN, 2) X(n_ioff, ioff_t, c.NN, 2)                                    \
   X(n_nsucc, uint8_t, c.NN, 0) X(n_nact, uint8_t, c.NN, 0) X(n_npred, uint8_t, c.NN, 0)                                \
-  X(n_sfreq, uint16_t, 4 * c.NN, 0) X(n_snid, uint16_t, 4 * c.NN, 0)                                                  \
+  X(n_sfreq, cnt_t, 4 * c.NN, 0) X(n_snid, uint16_t, 4 * c.NN, 0)                                                     \
   X(ipos, uint8_t, c.NI + c.EX, 2) X(irpos, uint8_t, c.NI + c.EX, 2)                                                  \
   X(ex_kmer, uint32_t, c.EX, 0) X(ex_pos, uint8_t, c.EX, 0) X(ex_rpos, uint8_t, c.EX, 0)                               \
-  X(ll_kmer, uint32_t, c.S, 0) X(ll_cnt, uint16_t, c.S, 0) X(fl_kmer, uint32_t, c.S, 0) X(fl_cnt, uint16_t, c.S, 0)    \
+  X(ll_kmer, uint32_t, c.S, 0) X(ll_cnt, cnt_t, c.S, 0) X(fl_kmer, uint32_t, c.S, 0) X(fl_cnt, cnt_t, c.S, 0)          \
   X(fl_nid, uint16_t, c.S, 0)                                                                                         \
   X(slinks, uint16_t, c.SL, 2) X(slsym, uint8_t, c.SL, 2) X(rs_off, uint16_t, c.ST, 0) X(rs_len, uint16_t, c.ST, 0)    \
   X(rs_fO, uint32_t, c.ST, 0) X(rs_cO, uint32_t, c.ST, 0) X(spc, uint32_t, 4, 0)                                       \
@@ -162,7 +184,11 @@ struct WS {
 #endif
   DCU_WS_FIELDS(X)
 #undef X
+#if DCU_WIDE
+  DCU_MEM uint32_t* fillcnt() const { return n_sfreq(); }     // per-node fill counters of build_nodes, 32 bit: the successor frequencies (4 NN) are rewritten by build_edges
+#else
   DCU_MEM uint16_t* fillcnt() const { return slinks(); }      // per-node fill counters of build_nodes: the link array is not in use while nodes are built (SL >= NN)
+#endif
 };
 
 // per-window state that all lanes hold identically
@@ -191,10 +217,20 @@ DCU_FN int hv_node(hval_t v) { return (v & 0x8000u) ? (int)(v & 0x7FFFu) : (int)
 DCU_FN hval_t hv_make(int cnt, int nid) { return nid == (int)NID_NONE ? (hval_t)cnt : (hval_t)(0x8000u | (uint32_t)nid); }
 // counts are 16-bit halves of 32-bit words: the add goes to the containing word (a count never reaches 2^15: HCAP / NI bound it)
 DCU_FN void hv_inc(hval_t* base, uint32_t h) { a_add((uint32_t*)base + (h >> 1), (h & 1u) ? 0x10000u : 1u); }      // (arrays are 16-byte aligned; indexing the word keeps the address space known: ATOMS, not a generic atomic)
+#elif DCU_WIDE
+DCU_FN int hv_node(hval_t v) { return (int)(v >> 32); }
+DCU_FN hval_t hv_make(int cnt, int nid) { return (hval_t)(uint32_t)cnt | ((hval_t)nid << 32); }
+DCU_FN void hv_inc(hval_t* base, uint32_t h) { a_add64(base + h, 1ull); }
 #else
 DCU_FN int hv_node(hval_t v) { return (int)(v >> 16); }
 DCU_FN hval_t hv_make(int cnt, int nid) { return (hval_t)cnt | ((hval_t)nid << 16); }
 DCU_FN void hv_inc(hval_t* base, uint32_t h) { a_add(base + h, 1u); }
+#endif
+// the count a slot value carries (build_nodes: slots hold counts or count | node id, never a bare node id)
+#if DCU_WIDE
+DCU_FN int hv_count(hval_t v) { return (int)(uint32_t)v; }
+#else
+DCU_FN int hv_count(hval_t v) { return (int)(v & 0xFFFFu); }
 #endif
 // 16-bit counter add on the containing 32-bit word; returns the old value of the half (no carry: the counters stay below 2^16)
 DCU_FN uint32_t add16(uint16_t* base, uint32_t i, uint32_t v) {
@@ -202,6 +238,12 @@ DCU_FN uint32_t add16(uint16_t* base, uint32_t i, uint32_t v) {
   const uint32_t o = a_add((uint32_t*)base + (i >> 1), hi ? (v << 16) : v);
   return hi ? (o >> 16) : (o & 0xFFFFu);
 }
+// next free instance slot of node n (build_nodes): the node's fill counter, 16 bit except in the wide build
+#if DCU_WIDE
+DCU_FN uint32_t fill_next(uint32_t* cnt, uint32_t n) { return a_add(cnt + n, 1u); }
+#else
+DCU_FN uint32_t fill_next(uint16_t* cnt, uint32_t n) { return add16(cnt, n, 1u); }
+#endif
 DCU_FN int lookup_from(const Ctx& c, uint32_t v, uint32_t h, uint32_t key) {      // key = hkey[h], already loaded
   const uint32_t mask = (1u << c.logh) - 1u;
   DCU_NOUNROLL
@@ -338,16 +380,16 @@ DCU_BIG void load_window(Ctx& c, const Window& win, int lane, const uint8_t* raw
       big = big || len > 255u;                         // slices are at most 255 bases (8-bit instance positions)
       const uint32_t nw = (len + 15u) >> 4;
       const uint32_t inc = scan_incl(len, lane), incw = scan_incl(nw, lane), incr = scan_incl(cb, lane);
-      if (j < c.MAo) { w.soff()[j] = (uint16_t)(run + inc - len); w.sw()[j] = (uint16_t)(runw + incw - nw); w.koff()[j] = (uint16_t)(runr + incr - cb); }      // koff: offsets of the staged chunks
+      if (j < c.MAo) { w.soff()[j] = (soff_t)(run + inc - len); w.sw()[j] = (soff_t)(runw + incw - nw); w.koff()[j] = (soff_t)(runr + incr - cb); }      // koff: offsets of the staged chunks
       run += bcast(inc, DCU_NL - 1); runw += bcast(incw, DCU_NL - 1); runr += bcast(incr, DCU_NL - 1);
     }
     if (ballot(big)) run = 0x10000000u;
-    if (lane == 0) { w.soff()[c.MAo] = (uint16_t)(run > 65535u ? 65535u : run); w.sw()[c.MAo] = (uint16_t)(runw > 65535u ? 65535u : runw); }
+    if (lane == 0) { w.soff()[c.MAo] = (soff_t)(run > DCU_OFF_MAX ? DCU_OFF_MAX : run); w.sw()[c.MAo] = (soff_t)(runw > DCU_OFF_MAX ? DCU_OFF_MAX : runw); }
     c.nbases = (int)(run > 0x0fffffffu ? 0x0fffffff : run);
   }
   wsync();
   DCU_PEAK(0, c.MAo); DCU_PEAK(1, c.nbases);
-  if (c.nbases > DCU_CAP.B || c.nbases > 65000 || (int)runw > DCU_CAP.BW) { c.overflow = 2; return; }
+  if (c.nbases > DCU_CAP.B || c.nbases > DCU_MAX_BASES || (int)runw > DCU_CAP.BW) { c.overflow = 2; return; }
   DCU_NOUNROLL
   for (int j = lane; j < c.MAo; j += DCU_NL) {
     const Slice s = sl[j];
@@ -415,7 +457,7 @@ DCU_BIG int estimate_length(Ctx& c, int lane) {
 // ------------------------------------------------------------------ k-mer hash build (replaces setupPreNodes :2018-2304)
 // sort a short (count, kmer[, node]) list descending by (count, kmer) -- std::greater on pairs (:1297-1301, :1384-1388);
 // k-mers are distinct, so the rank of an entry is the number of larger entries: lanes over entries
-DCU_BIG void rank_sort_desc(Ctx& c, uint32_t* km, uint16_t* cn, uint16_t* nd, int n, int lane) {
+DCU_BIG void rank_sort_desc(Ctx& c, uint32_t* km, cnt_t* cn, uint16_t* nd, int n, int lane) {
   const WS w = c.ws;
   // (count, kmer) as one 64-bit key (counts are >= 1, so 0 is below every entry); the other entries come by shuffle, 32 at a time
   DCU_NOUNROLL
@@ -430,7 +472,7 @@ DCU_BIG void rank_sort_desc(Ctx& c, uint32_t* km, uint16_t* cn, uint16_t* nd, in
       DCU_NOUNROLL
       for (int t = 0; t < cnt; ++t) r += bcast(theirs, t) > mine ? 1 : 0;
     }
-    if (e < n) { w.ts_k()[r] = (uint32_t)mine; w.ts_c()[r] = (uint16_t)(mine >> 32); if (nd) w.ts_n()[r] = nd[e]; }
+    if (e < n) { w.ts_k()[r] = (uint32_t)mine; w.ts_c()[r] = (cnt_t)(mine >> 32); if (nd) w.ts_n()[r] = nd[e]; }
   }
   wsync();
   DCU_NOUNROLL
@@ -619,7 +661,7 @@ DCU_BIG void build_hash(Ctx& c, int lane, bool pre) {
       }
       uint32_t bb = ballot(first);
       int idx = nl + popc(bb & lanemask_lt(lane));
-      if (first) { w.ll_kmer()[idx] = v; w.ll_cnt()[idx] = (uint16_t)cnt; }
+      if (first) { w.ll_kmer()[idx] = v; w.ll_cnt()[idx] = (cnt_t)cnt; }
       nl += popc(bb);
     }
     wsync();
@@ -646,13 +688,13 @@ DCU_BIG void build_nodes(Ctx& c, int f, int lane) {
   for (int base = 0; base < H; base += DCU_NL) {
     const int h = base + lane;                         // H is a multiple of 32
     const uint32_t key = nkey;
-    const int cnt = (int)(nval & 0xFFFFu);
+    const int cnt = hv_count(nval);
     if (base + DCU_NL < H) { nkey = w.hkey()[h + DCU_NL]; nval = w.hval()[h + DCU_NL]; }
     const bool occ = key != W_EMPTY, keep = occ && cnt >= f;
     const uint32_t b = ballot(keep);
     const int idx = nn + popc(b & lanemask_lt(lane));
     if (keep) {
-      if (idx < DCU_CAP.NN && idx < 0x7FFF) { w.n_kmer()[idx] = key; w.n_freq()[idx] = (uint16_t)cnt; w.hval()[h] = hv_make(cnt, idx); w.fillcnt()[idx] = 0; }
+      if (idx < DCU_CAP.NN && idx < 0x7FFF) { w.n_kmer()[idx] = key; w.n_freq()[idx] = (cnt_t)cnt; w.hval()[h] = hv_make(cnt, idx); w.fillcnt()[idx] = 0; }
     } else if (occ) w.hval()[h] = hv_make(cnt, NID_NONE);
     nn += popc(b);
   }
@@ -682,12 +724,12 @@ DCU_BIG void build_nodes(Ctx& c, int f, int lane) {
   // instances are filed under their nodes: the k-mers are rolled once more and looked up (no per-instance slot array)
   for_each_kmer_pf(c, lane, [&](uint32_t v) { return w.hkey()[hslot(c, v)]; }, [&](int, int i, int len, uint32_t v, uint32_t key) {
     const int n = lookup_fast(c, v, key);
-    if (n != NID_NONE) { const uint32_t t = add16(w.fillcnt(), (uint32_t)n, 1u) + (uint32_t)w.n_ioff()[n]; w.ipos()[t] = (uint8_t)i; w.irpos()[t] = (uint8_t)(len - i - c.k); }
+    if (n != NID_NONE) { const uint32_t t = fill_next(w.fillcnt(), (uint32_t)n) + (uint32_t)w.n_ioff()[n]; w.ipos()[t] = (uint8_t)i; w.irpos()[t] = (uint8_t)(len - i - c.k); }
   }, [](int, uint32_t) {});
   DCU_NOUNROLL
   for (int e = lane; e < c.nex; e += DCU_NL) {       // synthesised k-mers of the gap filler (:1148-1157)
     int n = lookup(c, w.ex_kmer()[e]);
-    if (n != NID_NONE) { const uint32_t t = add16(w.fillcnt(), (uint32_t)n, 1u) + (uint32_t)w.n_ioff()[n]; w.ipos()[t] = w.ex_pos()[e]; w.irpos()[t] = w.ex_rpos()[e]; }
+    if (n != NID_NONE) { const uint32_t t = fill_next(w.fillcnt(), (uint32_t)n) + (uint32_t)w.n_ioff()[n]; w.ipos()[t] = w.ex_pos()[e]; w.irpos()[t] = w.ex_rpos()[e]; }
   }
   wsync();
   uint32_t nf = 0;
@@ -711,7 +753,7 @@ DCU_BIG void build_nodes(Ctx& c, int f, int lane) {
     }
     uint32_t b = ballot(c0 > 0);               // k-mers seen at position 0 (maxForPosList :1280-1304)
     int idx = (int)nf + popc(b & lanemask_lt(lane));
-    if (c0 > 0 && idx < DCU_CAP.S) { w.fl_kmer()[idx] = w.n_kmer()[n]; w.fl_cnt()[idx] = (uint16_t)c0; w.fl_nid()[idx] = (uint16_t)n; }
+    if (c0 > 0 && idx < DCU_CAP.S) { w.fl_kmer()[idx] = w.n_kmer()[n]; w.fl_cnt()[idx] = (cnt_t)c0; w.fl_nid()[idx] = (uint16_t)n; }
     nf += popc(b);
   }
   wsync();
@@ -773,7 +815,7 @@ DCU_BIG void build_edges(Ctx& c, int lane) {
       while (na < ns && (((key[na] >> 8) >= (key[0] >> 8) / 2) || (DCU_P.check && (unsigned long long)(key[na] >> 8) >= lim))) ++na;
     }
     DCU_NOUNROLL
-    for (int e = 0; e < 4; ++e) { w.n_sfreq()[4 * n + e] = e < ns ? (uint16_t)(key[e] >> 8) : 0; w.n_snid()[4 * n + e] = e < ns ? nid[e] : (uint16_t)NID_NONE; }
+    for (int e = 0; e < 4; ++e) { w.n_sfreq()[4 * n + e] = e < ns ? (cnt_t)(key[e] >> 8) : 0; w.n_snid()[4 * n + e] = e < ns ? nid[e] : (uint16_t)NID_NONE; }
     w.n_nsucc()[n] = (uint8_t)ns; w.n_nact()[n] = (uint8_t)na;
   }
   wsync();
@@ -1995,3 +2037,6 @@ DCU_FN void process_window(Ctx& c, const Window& win, Result& res, uint8_t* cons
 #undef DCU_NS
 #undef DCU_TIER_SMEM
 #undef DCU_IN_SMEM
+#undef DCU_WIDE
+#undef DCU_OFF_MAX
+#undef DCU_MAX_BASES

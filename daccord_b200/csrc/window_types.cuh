@@ -28,6 +28,7 @@ namespace dcub {
 static inline void wsync() {}
 static inline uint32_t a_cas(uint32_t* p, uint32_t c, uint32_t v) { uint32_t o = *p; if (o == c) *p = v; return o; }
 static inline uint32_t a_add(uint32_t* p, uint32_t v) { uint32_t o = *p; *p = o + v; return o; }
+static inline unsigned long long a_add64(unsigned long long* p, unsigned long long v) { unsigned long long o = *p; *p = o + v; return o; }
 static inline uint32_t a_or(uint32_t* p, uint32_t v) { uint32_t o = *p; *p = o | v; return o; }
 static inline uint32_t a_load(const uint32_t* p) { return *p; }
 static inline uint32_t ballot(bool p) { return p ? 1u : 0u; }
@@ -57,6 +58,7 @@ static inline void wsync_line(int line) { if (line != emu_skip_sync_line) emu_xc
 #define wsync() wsync_line(__LINE__)
 static inline uint32_t a_cas(uint32_t* p, uint32_t c, uint32_t v) { __atomic_compare_exchange_n(p, &c, v, false, __ATOMIC_RELAXED, __ATOMIC_RELAXED); return c; }   // real atomics: the lanes are OS threads in the ThreadSanitizer build
 static inline uint32_t a_add(uint32_t* p, uint32_t v) { return __atomic_fetch_add(p, v, __ATOMIC_RELAXED); }
+static inline unsigned long long a_add64(unsigned long long* p, unsigned long long v) { return __atomic_fetch_add(p, v, __ATOMIC_RELAXED); }
 static inline uint32_t a_or(uint32_t* p, uint32_t v) { return __atomic_fetch_or(p, v, __ATOMIC_RELAXED); }
 static inline uint32_t a_load(const uint32_t* p) { return __atomic_load_n(p, __ATOMIC_RELAXED); }
 static inline uint32_t ballot(bool p) { const unsigned long long* x = emu_xchg(p ? 1 : 0); uint32_t m = 0; for (int i = 0; i < 32; ++i) if (x[i]) m |= 1u << i; return m; }
@@ -97,6 +99,7 @@ namespace dcub {
 __device__ __forceinline__ void wsync() { __syncwarp(); }
 __device__ __forceinline__ uint32_t a_cas(uint32_t* p, uint32_t c, uint32_t v) { return atomicCAS(p, c, v); }
 __device__ __forceinline__ uint32_t a_add(uint32_t* p, uint32_t v) { return atomicAdd(p, v); }
+__device__ __forceinline__ unsigned long long a_add64(unsigned long long* p, unsigned long long v) { return atomicAdd(p, v); }
 __device__ __forceinline__ uint32_t a_or(uint32_t* p, uint32_t v) { return atomicOr(p, v); }
 __device__ __forceinline__ uint32_t a_load(const uint32_t* p) { return *(const volatile uint32_t*)p; }      // a counter other lanes are adding to
 __device__ __forceinline__ uint32_t ballot(bool p) { return __ballot_sync(0xffffffffu, p); }

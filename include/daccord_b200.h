@@ -85,6 +85,16 @@ int dcu_set_reads(dcu_ctx* ctx, const uint8_t* packed, uint64_t nbytes);
 int dcu_set_reads_device(dcu_ctx* ctx, const void* dpacked, uint64_t nbytes);
 /* same database as `owner` (a dcu_ctx on the same device that got it through dcu_set_reads[_device]); owner must outlive ctx's use of it */
 int dcu_share_reads(dcu_ctx* ctx, dcu_ctx* owner);
+/* deepest window (slices, the A window included) the context computes a consensus for; 1 .. 65535 (the ABI's 16-bit slice_cnt), default 2047.
+ * Call it before dcu_upload / dcu_pile.  Windows with more slices end as DCU_WIN_OVERFLOW.  Above 2047:
+ *  - the k-mer limit table gets max_slices + 1 columns (its first 2048 are unchanged; dcu_get_tables(which = 5) reports the new KLIMN);
+ *    building it takes a moment on the host (DESIGN.md section 2);
+ *  - windows that still overflow after the large-workspace pass (more than 65 000 bases, or a graph beyond its capacities) are run once
+ *    more by a wide pass: 32-bit slice offsets and k-mer counts, free running, on slabs sized to the batch's largest window, allocated for
+ *    the pass and released after it.  The slabs of one context take at most 2 GiB; windows of more than 4 Mi bases, and every window
+ *    when not even one slab fits the budget or the allocation fails, keep DCU_WIN_OVERFLOW and count as lost (dcu_last_stats2).
+ * At 2047 or below nothing of this happens: the context behaves as one that never made the call. */
+int dcu_set_max_depth(dcu_ctx* ctx, uint32_t max_slices);
 /* run one batch: host buffers in, host buffers out (results in submission order).
  * cons must hold nwin*DCU_CONS_STRIDE bytes, ops nwin*DCU_OPS_STRIDE bytes. */
 int dcu_run(dcu_ctx* ctx, const dcu_window* win, uint64_t nwin, const dcu_slice* sl, uint64_t nsl,
@@ -129,6 +139,8 @@ int dcu_last_stats(dcu_ctx* ctx, uint64_t* launches, uint64_t* hard_windows);
  * (status DCU_WIN_OVERFLOW), warps per SM and shared-memory bytes per warp of a first pass that keeps data in shared memory (the hybrid
  * pass: k-mer table only, 32 warps; DCU_SMEM=1: the graph, 12-16 warps; 0 warps = plain HBM first pass) */
 int dcu_last_stats2(dcu_ctx* ctx, uint64_t* second_pass_windows, uint64_t* lost_windows, uint32_t* smem_warps, uint32_t* smem_bytes_per_warp);
+/* the wide pass of the last launch (see dcu_set_max_depth): windows it ran (0: no pass), its warps and the bytes of slab it allocated */
+int dcu_last_wide_stats(dcu_ctx* ctx, uint64_t* wide_windows, uint32_t* wide_warps, uint64_t* wide_slab_bytes);
 /* dump the tables the kernel reads, copied back from the device (for tests): which = 0 DPnorm, 1 DPnormSquare, 2 VS (dense [NP][MS]),
  * 3 support lo/hi interleaved, 4 k-mer limits ([k][KLIMN]), 5 NP, MS, KLIMN.  Returns the number of doubles written / needed (nothing is
  * copied when out is NULL or cap is too small), -1 on a CUDA error */
