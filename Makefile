@@ -9,7 +9,7 @@ CSRC     := daccord_b200/csrc
 NVFLAGS  := -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -fmad=false -Xcompiler -fPIC,-O3,-ffp-contract=off,-fopenmp -shared
 CXXFLAGS := -O3 -g -std=c++17 -march=x86-64-v2 -ffp-contract=off -fopenmp -pthread
 CUDEPS   := $(wildcard $(CSRC)/*.cu $(CSRC)/*.cuh $(CSRC)/*.hpp) include/daccord_b200.h
-HOSTDEPS := $(wildcard $(CSRC)/host/*.hpp $(CSRC)/host/*.cpp) include/daccord_b200.h
+HOSTDEPS := $(wildcard $(CSRC)/host/*.hpp $(CSRC)/host/*.cpp) $(CSRC)/profile_core.cuh include/daccord_b200.h
 
 all: $(B)/libdaccord_b200.so $(B)/libdaccord_host.so $(B)/daccord oracle
 

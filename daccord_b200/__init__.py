@@ -16,6 +16,8 @@ WINDOW_DT = np.dtype([("slice_begin", "<u4"), ("slice_cnt", "<u2"), ("reserved",
 RESULT_DT = np.dtype([("status", "u1"), ("k", "u1"), ("ff", "i1"), ("clen", "u1"), ("err", "<u4"), ("nops", "<u2"),
                       ("ncand", "<u2"), ("elength", "<i4")])
 SEGMENT_DT = np.dtype([("aread", "<u4"), ("first", "<u4"), ("last", "<u4"), ("reserved", "<u4"), ("len", "<u8"), ("off", "<u8")])
+PROFILE_WINDOW_DT = np.dtype([("aread", "<u4"), ("astart", "<u4"), ("status", "<u4"), ("reserved", "<u4"), ("cnt", "<u4", (4,))])
+PROF_SKIPPED, PROF_REPEAT, PROF_NO_CONSENSUS, PROF_OK = 0, 1, 2, 3
 CONS_STRIDE, OPS_STRIDE = 64, 128
 WIN_SKIPPED, WIN_OK, WIN_FAILED = 0, 1, 2
 
@@ -116,6 +118,20 @@ class Engine:
                                    C.c_uint64(len(read_len)), C.c_uint32(advance), C.c_uint64(maxalign), C.byref(nw), C.byref(ns)))
         self.nwin, self.nsl = nw.value, ns.value
         return nw.value, ns.value
+
+    def profile(self, ovl, trace, tspace, read_boff, read_len, maxalign=2**64 - 1):
+        """windows of the error-profile estimator on the GPU (dcu_profile): ovl = the estimator's overlap selection
+        (Dataset.overlaps(..., profile=True)); returns (records as PROFILE_WINDOW_DT, windows finished on the host).
+        Replaces the resident batch."""
+        n = C.c_uint64(0)
+        self._ck(self.lib.dcu_profile(self.ctx, _p(ovl), C.c_uint64(len(ovl)), _p(trace), C.c_uint64(len(trace)), C.c_int32(tspace), _p(read_boff), _p(read_len),
+                                      C.c_uint64(len(read_len)), C.c_uint64(maxalign), C.byref(n)))
+        self.nwin = self.nsl = 0
+        rec = np.zeros(n.value, PROFILE_WINDOW_DT)
+        self._ck(self.lib.dcu_get_profile(self.ctx, _p(rec)))
+        h = C.c_uint64(0)
+        self._ck(self.lib.dcu_last_profile_stats(self.ctx, C.byref(h)))
+        return rec, h.value
 
     def get_windows(self, with_slices=False):
         win = np.zeros(self.nwin, WINDOW_DT)

@@ -27,7 +27,8 @@ def build(force=False, verbose=False):
         env["PATH"] = "/usr/bin:" + env.get("PATH", "")      # system g++ (the /opt/gcc wrapper lacks libgomp.spec)
         subprocess.check_call(cmd, env=env)
     host_src = os.path.join(csrc, "host", "hostlib.cpp")  # noqa
-    host_deps = [os.path.join(csrc, "host", f) for f in os.listdir(os.path.join(csrc, "host"))] + [os.path.join(ROOT, "include", "daccord_b200.h")]
+    host_deps = [os.path.join(csrc, "host", f) for f in os.listdir(os.path.join(csrc, "host"))] + [os.path.join(ROOT, "include", "daccord_b200.h"),
+                                                                                               os.path.join(csrc, "profile_core.cuh")]
     if force or _newer(HOST_LIB, host_deps):
         subprocess.check_call(["/usr/bin/g++", "-O3", "-g", "-std=c++17", "-march=x86-64-v2", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared",
                                "-o", HOST_LIB, host_src])

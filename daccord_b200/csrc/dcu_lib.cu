@@ -29,6 +29,7 @@
 #include "host_caps.hpp"
 #include "pile_host.hpp"
 #include "vote_host.hpp"
+#include "profile_core.cuh"           // namespace dprof: one window of the error-profile estimator (dcu_profile)
 #include "../../include/daccord_b200.h"
 
 static_assert(sizeof(dcu::Slice) == sizeof(dcu_slice) && sizeof(dcu::Window) == sizeof(dcu_window) && sizeof(dcu::Result) == sizeof(dcu_result), "ABI structs");
@@ -356,16 +357,18 @@ __global__ void pile_k2a(const dpile::ReadInfo* reads, uint64_t nr, const dpile:
 }
 // one thread per candidate window.  pass 0 (win == nullptr): slices per candidate (0 = empty pile) and per block the number of
 // windows and slices; pass 1: descriptors at the scanned offsets
-__global__ void __launch_bounds__(VOTE_TPB) pile_k2(const dpile::ReadInfo* reads, const uint32_t* read_id, uint32_t nr, uint64_t ncand, const dpile::Ovl* ovl, dpile::Params P,
-                                                   const uint32_t* bm, const uint64_t* read_boff, const uint32_t* read_len, const unsigned long long* keys,
-                                                   uint32_t* cnt, uint64_t* blkw, uint64_t* blks, dpile::Win* win, dpile::Sl* sl, int* err) {
+// (PROF: the piles of the error-profile estimator, pile_k2p)
+template <bool PROF>
+__device__ __forceinline__ void pile_k2_body(const dpile::ReadInfo* reads, const uint32_t* read_id, uint32_t nr, uint64_t ncand, const dpile::Ovl* ovl, const dpile::Params& P,
+                                             const uint32_t* bm, const uint64_t* read_boff, const uint32_t* read_len, const unsigned long long* keys,
+                                             uint32_t* cnt, uint64_t* blkw, uint64_t* blks, dpile::Win* win, dpile::Sl* sl, int* err) {
   const uint64_t idx = (uint64_t)blockIdx.x * VOTE_TPB + threadIdx.x;
   uint32_t n = 0, r = 0, y = 0;
   if (idx < ncand) {
     uint32_t a = 0, b = nr;                       // last read with win_off <= idx that has candidates
     while (b - a > 1) { uint32_t mid = (a + b) >> 1; if (reads[mid].win_off <= idx) a = mid; else b = mid; }
     r = a; y = (uint32_t)(idx - reads[r].win_off);
-    if (!win) { n = (uint32_t)dpile::pile_window(reads[r], y, ovl, P, bm, read_boff, read_len, keys + reads[r].ovl_begin, read_id[r], nullptr, nullptr, 0u); cnt[idx] = n; }
+    if (!win) { n = (uint32_t)dpile::pile_window_m<PROF>(reads[r], y, ovl, P, bm, read_boff, read_len, keys + reads[r].ovl_begin, read_id[r], nullptr, nullptr, 0u); cnt[idx] = n; }
     else n = cnt[idx];
   }
   uint32_t totw, tots;
@@ -374,8 +377,14 @@ __global__ void __launch_bounds__(VOTE_TPB) pile_k2(const dpile::ReadInfo* reads
   if (!win) { if (threadIdx.x == 0) { blkw[blockIdx.x] = totw; blks[blockIdx.x] = tots; } return; }
   if (!n) return;
   const uint64_t wo = blkw[blockIdx.x] + woff, so = blks[blockIdx.x] + soff;
-  if (dpile::pile_window(reads[r], y, ovl, P, bm, read_boff, read_len, keys + reads[r].ovl_begin, read_id[r], win + wo, sl + so, (uint32_t)so) < 0) atomicExch(err, 2);
+  if (dpile::pile_window_m<PROF>(reads[r], y, ovl, P, bm, read_boff, read_len, keys + reads[r].ovl_begin, read_id[r], win + wo, sl + so, (uint32_t)so) < 0) atomicExch(err, 2);
 }
+#define PILE_K2_ARGS const dpile::ReadInfo* reads, const uint32_t* read_id, uint32_t nr, uint64_t ncand, const dpile::Ovl* ovl, dpile::Params P, const uint32_t* bm, \
+                     const uint64_t* read_boff, const uint32_t* read_len, const unsigned long long* keys, uint32_t* cnt, uint64_t* blkw, uint64_t* blks,       \
+                     dpile::Win* win, dpile::Sl* sl, int* err
+__global__ void __launch_bounds__(VOTE_TPB) pile_k2(PILE_K2_ARGS) { pile_k2_body<false>(reads, read_id, nr, ncand, ovl, P, bm, read_boff, read_len, keys, cnt, blkw, blks, win, sl, err); }
+__global__ void __launch_bounds__(VOTE_TPB) pile_k2p(PILE_K2_ARGS) { pile_k2_body<true>(reads, read_id, nr, ncand, ovl, P, bm, read_boff, read_len, keys, cnt, blkw, blks, win, sl, err); }
+#undef PILE_K2_ARGS
 // per-window pile statistics of a device-built batch: max slice count and max bases of a window
 __global__ void pile_k3(const dpile::Win* win, const dpile::Sl* sl, uint64_t nwin, unsigned int* maxS, unsigned int* maxB) {
   uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -383,6 +392,42 @@ __global__ void pile_k3(const dpile::Win* win, const dpile::Sl* sl, uint64_t nwi
   const dpile::Win w = win[i]; unsigned int b = 0;
   for (uint32_t j = 0; j < w.slice_cnt; ++j) b += sl[w.slice_begin + j].len;
   atomicMax(maxS, (unsigned int)w.slice_cnt); atomicMax(maxB, b);
+}
+
+// ---- error-profile windows (profile_core.cuh): one thread per window, grid-stride, each thread on its own PROF_SCRATCH bytes of HBM
+// scratch of prof_scratch_bytes (the hash table, marks and 7-mer bits start zeroed and are left zeroed by every window)
+constexpr int PROF_TPB = 128, PROF_BLOCKS_PER_SM = 2;
+// decodes the slices of window w into S (false: beyond S's capacities)
+__host__ __device__ inline bool prof_load(const dpile::Win& w, const dpile::Sl* sl, const uint8_t* packed, const dprof::Scratch& S) {
+  if (w.slice_cnt > S.maxs) return false;
+  uint32_t tot = 0;
+  for (uint32_t j = 0; j < w.slice_cnt; ++j) { const uint32_t len = sl[w.slice_begin + j].len; if (len > S.maxlen) return false; tot += len; }
+  if (tot > S.maxb) return false;
+  uint32_t o = 0;
+  for (uint32_t j = 0; j < w.slice_cnt; ++j) {
+    const dpile::Sl x = sl[w.slice_begin + j]; S.soff[j] = o;
+    for (uint32_t i = 0; i < x.len; ++i) {
+      const uint32_t g = (x.flags & 1u) ? x.gpos + x.len - 1 - i : x.gpos + i;
+      const uint8_t b = (packed[g >> 2] >> (6 - 2 * (g & 3))) & 3;
+      S.bases[o++] = (x.flags & 1u) ? (uint8_t)(3 - b) : b;
+    }
+  }
+  S.soff[w.slice_cnt] = o;
+  return true;
+}
+__global__ void __launch_bounds__(PROF_TPB) prof_k(const dpile::Win* win, const dpile::Sl* sl, uint64_t nwin, const uint8_t* packed, uint8_t* scratch,
+                                                  uint64_t stride, dcu_profile_window* out) {
+  const uint64_t tid = (uint64_t)blockIdx.x * PROF_TPB + threadIdx.x, nth = (uint64_t)gridDim.x * PROF_TPB;
+  if (tid >= nwin) return;
+  const dprof::Scratch S = dprof::scratch_at(scratch + tid * stride, dprof::PROF_MAXS, dprof::PROF_MAXB, dprof::PROF_HSZ, dprof::PROF_MAXLEN);
+  for (uint64_t i = tid; i < nwin; i += nth) {
+    const dpile::Win w = win[i];
+    uint32_t g[4] = {0, 0, 0, 0}; int st = dprof::ST_SKIPPED;
+    if (w.slice_cnt >= 3) st = prof_load(w, sl, packed, S) ? dprof::prof_window(w.slice_cnt, S, g) : dprof::ST_HOST;
+    dcu_profile_window r; r.aread = w.aread; r.astart = w.astart; r.status = (uint32_t)st; r.reserved = 0;
+    for (int q = 0; q < 4; ++q) r.cnt[q] = g[q];
+    out[i] = r;
+  }
 }
 
 // ---- pile vote (vote_core.cuh): per window the offset table, per A position the column votes (count pass, then fill pass)
@@ -480,6 +525,10 @@ struct dcu_ctx {
   dcu_window* hwin = nullptr; uint64_t hwin_cap = 0;      // pinned host copy of the window descriptors (dcu_vote lays out the reads from it)
   unsigned int launch_seq = 0;
   uint64_t launches = 0, hard = 0, second = 0, lost = 0;     // second: windows the shared-memory pass handed on; hard: windows of the large-workspace pass; lost: beyond every capacity
+  // error-profile windows (dcu_profile): per-thread scratch, records, host copy of the read database for the windows finished on the host
+  DevBuf<uint8_t> dprof_scratch; DevBuf<dcu_profile_window> dprof_out;
+  std::vector<dcu_profile_window> prof; uint64_t prof_host = 0;
+  std::vector<uint8_t> hpacked; const uint8_t* hpacked_src = nullptr;
   std::string err;
 };
 
@@ -555,7 +604,7 @@ void dcu_destroy(dcu_ctx* ctx) {
   ctx->dpo.release(); ctx->dpr.release(); ctx->dprid.release(); ctx->dptile.release(); ctx->dpbm.release(); ctx->dprlen.release();
   ctx->dpboff.release(); ctx->dptrace.release(); ctx->dpmin.release(); ctx->dpdiv.release(); ctx->dpact.release(); ctx->dpcnt.release(); ctx->dpblkw.release(); ctx->dpblks.release();
   ctx->dovf[0].release(); ctx->dovf[1].release(); ctx->dovf[2].release(); ctx->dcnt.release(); ctx->dslab[0].release(); ctx->dslab[1].release(); ctx->dslab[2].release();
-  ctx->dslabH.release(); ctx->dovfH.release(); ctx->dvent.release(); ctx->dvflag.release(); ctx->dvblk.release(); ctx->dvchars.release(); ctx->dvreads.release(); ctx->dvbound.release();
+  ctx->dprof_scratch.release(); ctx->dprof_out.release(); ctx->dslabH.release(); ctx->dovfH.release(); ctx->dvent.release(); ctx->dvflag.release(); ctx->dvblk.release(); ctx->dvchars.release(); ctx->dvreads.release(); ctx->dvbound.release();
   if (ctx->hwin) cudaFreeHost(ctx->hwin);
   if (ctx->ev0) cudaEventDestroy(ctx->ev0);
   if (ctx->ev1) cudaEventDestroy(ctx->ev1);
@@ -697,15 +746,17 @@ int dcu_upload(dcu_ctx* ctx, const dcu_window* win, uint64_t nwin, const dcu_sli
   return DCU_OK;
 }
 
-// trace reconstruction + window / slice extraction on the device (pile_core.cuh)
-int dcu_pile(dcu_ctx* ctx, const dcu_overlap* ovl, uint64_t novl, const uint16_t* trace, uint64_t ntrace, int32_t tspace,
-             const uint64_t* read_boff, const uint32_t* read_len, uint64_t nreads, uint32_t advance, uint64_t maxalign, uint64_t* nwin_out, uint64_t* nsl_out) {
+// trace reconstruction + window / slice extraction on the device (pile_core.cuh) into ctx->dwin / ctx->dsl: windows of w bases advancing
+// by `advance`, the main loop's piles, or the error-profile estimator's with prof (pile_k2p)
+static int pile_impl(dcu_ctx* ctx, const dcu_overlap* ovl, uint64_t novl, const uint16_t* trace, uint64_t ntrace, int32_t tspace,
+                     const uint64_t* read_boff, const uint32_t* read_len, uint64_t nreads, uint32_t w, uint32_t advance, uint64_t maxalign, bool prof,
+                     uint64_t* nwin_out, uint64_t* nsl_out, unsigned int mx[2]) {
   if (!ctx || (!ovl && novl) || (!trace && ntrace) || !read_boff || !read_len) return DCU_ERR_PARAM;
   if (!ctx->dpacked) { ctx->err = "dcu_set_reads not called"; return DCU_ERR_STATE; }
   CK(cudaSetDevice(ctx->device));
-  Laps laps("dcu_pile");
+  Laps laps(prof ? "dcu_profile piling" : "dcu_pile");
   dpile::Prep P;
-  if (!dpile::prepare(ovl, novl, ntrace, tspace, ctx->prm.w, advance, nreads, read_len, P)) { ctx->err = P.err; return DCU_ERR_UNSUPPORTED; }
+  if (!dpile::prepare(ovl, novl, ntrace, tspace, w, advance, nreads, read_len, P, prof)) { ctx->err = P.err; return DCU_ERR_UNSUPPORTED; }
   laps.lap("prepare");
   int bad = 0;                                   // every B block must lie inside its read and fit the tile aligner
 #pragma omp parallel for schedule(static) reduction(max : bad)
@@ -721,7 +772,7 @@ int dcu_pile(dcu_ctx* ctx, const dcu_overlap* ovl, uint64_t novl, const uint16_t
   if (bad == 2) { ctx->err = "trace points run past the B read"; return DCU_ERR_PARAM; }
   if (bad == 1) { ctx->err = "read outside the packed database"; return DCU_ERR_PARAM; }
   const uint64_t nr = P.reads.size();
-  dpile::Params prm; prm.tspace = tspace; prm.w = ctx->prm.w; prm.a = advance; prm.maxalign = maxalign;
+  dpile::Params prm; prm.tspace = tspace; prm.w = w; prm.a = advance; prm.maxalign = maxalign;
   CK(ctx->dpo.ensure(novl + 1)); CK(ctx->dpr.ensure(nr + 1)); CK(ctx->dprid.ensure(nr + 1)); CK(ctx->dptile.ensure(P.ntiles + 1)); CK(ctx->dpbm.ensure(P.nbm + 1));
   CK(ctx->dprlen.ensure(nreads + 1)); CK(ctx->dpboff.ensure(nreads + 1)); CK(ctx->dptrace.ensure(ntrace + 1));
   CK(ctx->dpmin.ensure(nr + 1)); CK(ctx->dpdiv.ensure(nr + 1)); CK(ctx->dpact.ensure(novl + 1)); CK(ctx->dcnt.ensure(16));
@@ -738,7 +789,8 @@ int dcu_pile(dcu_ctx* ctx, const dcu_overlap* ovl, uint64_t novl, const uint16_t
     CK(cudaMemcpyAsync(ctx->dpdiv.p, P.ediv.data(), nr * 8, cudaMemcpyHostToDevice, st));
   }
   uint64_t tw = 0, ts = 0;
-  unsigned int mx[2] = {4, 64};
+  mx[0] = 4; mx[1] = 64;
+  auto k2 = prof ? pile_k2p : pile_k2;
   if (novl) {
     int* derr = (int*)(ctx->dcnt.p + 4);
     const uint64_t ncand = P.ncand, nblk = (ncand + VOTE_TPB - 1) / VOTE_TPB;
@@ -749,8 +801,8 @@ int dcu_pile(dcu_ctx* ctx, const dcu_overlap* ovl, uint64_t novl, const uint16_t
     pile_k1<<<(unsigned)((P.ntiles + 63) / 64), 64, 0, st>>>(ctx->dpo.p, novl, P.ntiles, ctx->dpr.p, prm, ctx->dptrace.p, ctx->dptile.p, ctx->dpacked, ctx->dpboff.p, ctx->dprlen.p, ctx->dpbm.p);
     pile_k2a<<<(unsigned)((nr + 63) / 64), 64, 0, st>>>(ctx->dpr.p, nr, ctx->dpo.p, ctx->dpmin.p, ctx->dpdiv.p, ctx->dpact.p);
     if (ncand) {
-      pile_k2<<<(unsigned)nblk, VOTE_TPB, 0, st>>>(ctx->dpr.p, ctx->dprid.p, (uint32_t)nr, ncand, ctx->dpo.p, prm, ctx->dpbm.p, ctx->dpboff.p, ctx->dprlen.p, ctx->dpact.p,
-                                                 ctx->dpcnt.p, ctx->dpblkw.p, ctx->dpblks.p, nullptr, nullptr, derr);
+      k2<<<(unsigned)nblk, VOTE_TPB, 0, st>>>(ctx->dpr.p, ctx->dprid.p, (uint32_t)nr, ncand, ctx->dpo.p, prm, ctx->dpbm.p, ctx->dpboff.p, ctx->dprlen.p, ctx->dpact.p,
+                                            ctx->dpcnt.p, ctx->dpblkw.p, ctx->dpblks.p, nullptr, nullptr, derr);
       vote_kscan<<<1, VOTE_TPB, 0, st>>>(ctx->dpblkw.p, nblk);
       vote_kscan<<<1, VOTE_TPB, 0, st>>>(ctx->dpblks.p, nblk);
       CK(cudaGetLastError());
@@ -762,14 +814,14 @@ int dcu_pile(dcu_ctx* ctx, const dcu_overlap* ovl, uint64_t novl, const uint16_t
     }
     if (tw >= 0xFFFFFFF0ull || ts >= 0xFFFFFFF0ull) { ctx->err = "batch too large"; return DCU_ERR_UNSUPPORTED; }
     CK(ctx->dwin.ensure(tw + 1)); CK(ctx->dsl.ensure(ts + 1));
-    if (tw) pile_k2<<<(unsigned)nblk, VOTE_TPB, 0, st>>>(ctx->dpr.p, ctx->dprid.p, (uint32_t)nr, ncand, ctx->dpo.p, prm, ctx->dpbm.p, ctx->dpboff.p, ctx->dprlen.p, ctx->dpact.p,
-                                                       ctx->dpcnt.p, ctx->dpblkw.p, ctx->dpblks.p, (dpile::Win*)ctx->dwin.p, (dpile::Sl*)ctx->dsl.p, derr);
+    if (tw) k2<<<(unsigned)nblk, VOTE_TPB, 0, st>>>(ctx->dpr.p, ctx->dprid.p, (uint32_t)nr, ncand, ctx->dpo.p, prm, ctx->dpbm.p, ctx->dpboff.p, ctx->dprlen.p, ctx->dpact.p,
+                                                  ctx->dpcnt.p, ctx->dpblkw.p, ctx->dpblks.p, (dpile::Win*)ctx->dwin.p, (dpile::Sl*)ctx->dsl.p, derr);
     unsigned int* dmx = ctx->dcnt.p + 6;
-    CK(cudaMemcpyAsync(dmx, mx, sizeof(mx), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(dmx, mx, 2 * sizeof(unsigned int), cudaMemcpyHostToDevice, st));
     if (tw) pile_k3<<<(unsigned)((tw + 255) / 256), 256, 0, st>>>((const dpile::Win*)ctx->dwin.p, (const dpile::Sl*)ctx->dsl.p, tw, dmx, dmx + 1);
     CK(cudaGetLastError());
     int herr = 0;
-    CK(cudaMemcpyAsync(mx, dmx, sizeof(mx), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(mx, dmx, 2 * sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(&herr, derr, 4, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     laps.lap("pass2+sync");
@@ -777,7 +829,89 @@ int dcu_pile(dcu_ctx* ctx, const dcu_overlap* ovl, uint64_t novl, const uint16_t
   }
   if (nwin_out) *nwin_out = tw;
   if (nsl_out) *nsl_out = ts;
+  return DCU_OK;
+}
+int dcu_pile(dcu_ctx* ctx, const dcu_overlap* ovl, uint64_t novl, const uint16_t* trace, uint64_t ntrace, int32_t tspace,
+             const uint64_t* read_boff, const uint32_t* read_len, uint64_t nreads, uint32_t advance, uint64_t maxalign, uint64_t* nwin_out, uint64_t* nsl_out) {
+  uint64_t tw = 0, ts = 0; unsigned int mx[2];
+  const int rc = pile_impl(ctx, ovl, novl, trace, ntrace, tspace, read_boff, read_len, nreads, ctx ? ctx->prm.w : 0, advance, maxalign, false, &tw, &ts, mx);
+  if (rc) return rc;
+  if (nwin_out) *nwin_out = tw;
+  if (nsl_out) *nsl_out = ts;
   return finish_batch(ctx, (int)mx[0], (int)mx[1], ts, tw, ts);
+}
+
+// error-profile windows: the estimator's piles (pile_k2p), then one thread per window (prof_k); windows beyond the device scratch come
+// back as ST_HOST and are run here by the same prof_window on scratch sized to them.  Records land in ctx->prof, in window order.
+int dcu_profile(dcu_ctx* ctx, const dcu_overlap* ovl, uint64_t novl, const uint16_t* trace, uint64_t ntrace, int32_t tspace,
+                const uint64_t* read_boff, const uint32_t* read_len, uint64_t nreads, uint64_t maxalign, uint64_t* nrec) {
+  if (!ctx) return DCU_ERR_PARAM;
+  ctx->prof.clear(); ctx->prof_host = 0;
+  uint64_t tw = 0, ts = 0; unsigned int mx[2];
+  int rc = pile_impl(ctx, ovl, novl, trace, ntrace, tspace, read_boff, read_len, nreads, 40, 5, maxalign, true, &tw, &ts, mx);
+  if (rc) return rc;
+  // the piles of dcu_profile are not a resident batch of the window kernel
+  ctx->nwin = 0; ctx->nsl = 0; ctx->results_valid = false;
+  Laps laps("dcu_profile");
+  ctx->prof.resize(tw);
+  if (tw) {
+    const size_t stride = dprof::scratch_bytes(dprof::PROF_MAXS, dprof::PROF_MAXB, dprof::PROF_HSZ, dprof::PROF_MAXLEN);
+    const uint64_t nth = std::min<uint64_t>((tw + PROF_TPB - 1) / PROF_TPB * PROF_TPB, (uint64_t)ctx->num_sms * PROF_BLOCKS_PER_SM * PROF_TPB);
+    CK(ctx->dprof_scratch.ensure(nth * stride, true)); CK(ctx->dprof_out.ensure(tw));
+    prof_k<<<(unsigned)(nth / PROF_TPB), PROF_TPB, 0, ctx->stream>>>((const dpile::Win*)ctx->dwin.p, (const dpile::Sl*)ctx->dsl.p, tw, ctx->dpacked,
+                                                                    ctx->dprof_scratch.p, stride, ctx->dprof_out.p);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(ctx->prof.data(), ctx->dprof_out.p, tw * sizeof(dcu_profile_window), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    laps.lap("kernel");
+    std::vector<uint64_t> todo;
+    for (uint64_t i = 0; i < tw; ++i) if (ctx->prof[i].status == dprof::ST_HOST) todo.push_back(i);
+    if (!todo.empty()) {
+      std::vector<dpile::Win> win(tw); std::vector<dpile::Sl> sl(ts);
+      CK(cudaMemcpy(win.data(), ctx->dwin.p, tw * sizeof(dpile::Win), cudaMemcpyDeviceToHost));
+      CK(cudaMemcpy(sl.data(), ctx->dsl.p, ts * sizeof(dpile::Sl), cudaMemcpyDeviceToHost));
+      if (ctx->hpacked_src != ctx->dpacked || ctx->hpacked.size() != ctx->packed_bytes) {
+        ctx->hpacked.resize(ctx->packed_bytes);
+        CK(cudaMemcpy(ctx->hpacked.data(), ctx->dpacked, ctx->packed_bytes, cudaMemcpyDeviceToHost));
+        ctx->hpacked_src = ctx->dpacked;
+      }
+      bool bad = false;
+#pragma omp parallel for schedule(dynamic, 1) reduction(|| : bad)
+      for (int64_t t = 0; t < (int64_t)todo.size(); ++t) {
+        const dpile::Win& w = win[todo[t]];
+        uint32_t tot = 0, ml = 0;
+        for (uint32_t j = 0; j < w.slice_cnt; ++j) { tot += sl[w.slice_begin + j].len; ml = std::max<uint32_t>(ml, sl[w.slice_begin + j].len); }
+        uint32_t hsz = 16; while (hsz < 2 * tot + 2) hsz <<= 1;
+        std::vector<uint8_t> buf(dprof::scratch_bytes(w.slice_cnt, tot, hsz, ml) + 16, 0);
+        dprof::Scratch S = dprof::scratch_at((uint8_t*)(((uintptr_t)buf.data() + 15) & ~(uintptr_t)15), w.slice_cnt, tot, hsz, ml);
+        uint32_t g[4];
+        int st = prof_load(w, sl.data(), ctx->hpacked.data(), S) ? dprof::prof_window(w.slice_cnt, S, g) : dprof::ST_HOST;
+        std::vector<int32_t> dp;
+        if (st == dprof::ST_HOST) {           // a consensus longer than 128 bases: once more with a DP matrix (at most tot + 8 consensus bases)
+          dp.resize((size_t)(ml + 1) * (tot + 9)); S.dp = dp.data(); S.dp_cap = dp.size();
+          st = dprof::prof_window(w.slice_cnt, S, g);
+        }
+        if (st == dprof::ST_HOST) { bad = true; continue; }
+        dcu_profile_window& r = ctx->prof[todo[t]];
+        r.status = (uint32_t)st; for (int q = 0; q < 4; ++q) r.cnt[q] = g[q];
+      }
+      if (bad) { ctx->err = "a profile window exceeded the host scratch"; return DCU_ERR_OVERFLOW; }
+      ctx->prof_host = todo.size();
+      laps.lap("host windows");
+    }
+  }
+  if (nrec) *nrec = tw;
+  return DCU_OK;
+}
+int dcu_get_profile(dcu_ctx* ctx, dcu_profile_window* rec) {
+  if (!ctx || (!rec && !ctx->prof.empty())) return DCU_ERR_PARAM;
+  if (!ctx->prof.empty()) memcpy(rec, ctx->prof.data(), ctx->prof.size() * sizeof(dcu_profile_window));
+  return DCU_OK;
+}
+int dcu_last_profile_stats(dcu_ctx* ctx, uint64_t* host_windows) {
+  if (!ctx) return DCU_ERR_PARAM;
+  if (host_windows) *host_windows = ctx->prof_host;
+  return DCU_OK;
 }
 
 int dcu_get_windows(dcu_ctx* ctx, dcu_window* win, dcu_slice* sl) {

@@ -36,7 +36,8 @@ static const char* HELP =
     "\treads2.db: B-reads of an asymmetric alignment (daligner reads.db reads2.db); default reads.db\n"
     "\t-t: number of host threads (default: all)\n\t-w: window size (default 40)\n\t-a: advance size (default 10)\n"
     "\t-d: max depth (default unlimited)\n\t-f: produce full sequences\n\t-V: verbosity\n\t-I: read interval i,j (inclusive)\n"
-    "\t-J: reads part i,j\n\t-E: error profile file name (default input.las.eprof)\n\t--eprofonly: compute error profile only\n\t--keepeprof: keep an error profile older than the .las (default 1)\n\t-m: minimum window coverage (default 3)\n"
+    "\t-J: reads part i,j\n\t-E: error profile file name (default input.las.eprof)\n\t--eprofonly: compute error profile only\n"
+    "\t--deepprofileonly: print the distribution of the per-window error rates of the first 4096 reads of the range and exit\n\t--keepeprof: keep an error profile older than the .las (default 1)\n\t-m: minimum window coverage (default 3)\n"
     "\t-e: maximum window error (default unlimited)\n\t-l: minimum length of output (default 0)\n"
     "\t--minfilterfreq: minimum k-mer filter frequency (default 0)\n\t--maxfilterfreq: maximum k-mer filter frequency (default 2)\n"
     "\t-D: maximum number of alignments considered per read (default 5000)\n"
@@ -73,7 +74,7 @@ int main(int argc, char** argv) {
   // reads.las reads.db [reads2.db]: A-reads from reads.db, B-reads from reads2.db (reference src/daccord.cpp:2598-2622, :1337-1369)
   const std::string lasfn = A.pos[0], dbfn = A.pos[1], db2fn = A.pos.size() > 2 ? A.pos[2] : dbfn;
   const bool asym = db2fn != dbfn;
-  if (A.opt.count("deepprofileonly")) { fprintf(stderr, "[E] --deepprofileonly is not supported by this build\n"); return EXIT_FAILURE; }
+  const bool deep = A.opt.count("deepprofileonly") != 0;
   const uint64_t vard = getu("vard", 0);                                 // replaces -D when set (src/daccord.cpp:2121-2126)
   if (vard && asym) { fprintf(stderr, "[E] --vard is not supported for asymmetric (DB1 != DB2) alignments\n"); return EXIT_FAILURE; }     // :1340-1348
   dcu_params prm; memset(&prm, 0, sizeof(prm));
@@ -116,7 +117,8 @@ int main(int argc, char** argv) {
     }
     const int64_t toparead = maxaread >= 0 ? maxaread + 1 : maxaread;
     fprintf(stderr, "[V] minaread=%ld toparead=%ld\n", (long)minaread, (long)toparead);
-    fprintf(stderr, "[V] loading %s ...", lasfn.c_str()); read_las_range(lasfn, lidx, minaread, toparead, las, nthreads); las.build_index(nA);
+    const int64_t lastop = deep ? std::min<int64_t>(toparead, minaread + 4096) : toparead;      // --deepprofileonly: at most 4096 reads (:1467)
+    fprintf(stderr, "[V] loading %s ...", lasfn.c_str()); read_las_range(lasfn, lidx, minaread, lastop, las, nthreads); las.build_index(nA);
     validate_las(las, db.rlen, asym ? &db2.rlen : nullptr);
     if (asym) {       // one read space: reads2.db's reads follow reads.db's, so bread moves up by nA (LAS order, and so C6, unchanged)
       for (auto& o : las.ovl) o.bread += (int32_t)nA;
@@ -124,6 +126,52 @@ int main(int argc, char** argv) {
     }
     fprintf(stderr, "done (%zu of %ld overlaps).\n", las.ovl.size(), (long)lidx.novl);
     lap("inputs loaded");
+    if (deep) {
+      // --deepprofileonly (reference src/daccord.cpp:1442-1650): the error-profile estimator's windows over A-reads [minaread, lastop), the
+      // error rate of every window with a consensus, printed as its cumulative distribution; no error profile is read or written.
+      // The windows run on the GPU (dcu_profile) in batches of --batchreads reads; DACCORD_HOST_PROFILE=1, or trace tiles longer than the GPU
+      // piler takes, run them on the host (eprof.hpp)
+      std::vector<uint32_t> vals;
+      const bool host_prof = getenv("DACCORD_HOST_PROFILE") != nullptr;
+      if (host_prof || las.tspace > 128) {
+        if (!host_prof) fprintf(stderr, "[W] the profile windows run on the host for this input (the GPU piler aligns trace tiles of at most 128 A bases; here tspace=%d)\n", las.tspace);
+        for (const ProfileWindow& r : profile_windows(db, las, minaread, lastop, maxalign, maxinput, nthreads, vard, avglen, false, nullptr))
+          if (r.status == DCU_PROF_OK) vals.push_back(deep_value(r.cnt));
+      } else {
+        dcu_params pp; memset(&pp, 0, sizeof(pp));
+        pp.w = 40; pp.k_lo = pp.k_hi = 8; pp.min_cov = 3; pp.min_ff = 0; pp.max_ff = 2; pp.max_err = UINT64_MAX; pp.p_i = 0.09; pp.p_d = 0.045; pp.est_cor = 0.85;
+        dcu_ctx* ctx = nullptr;
+        int rc = dcu_create(&pp, device, &ctx);
+        if (!rc) rc = dcu_set_reads(ctx, db.bytes.data(), db.bytes.size());
+        if (rc) { fprintf(stderr, "[E] dcu_create / dcu_set_reads: %s %s\n", dcu_strerror(rc), ctx ? dcu_last_error(ctx) : ""); return EXIT_FAILURE; }
+        uint64_t tothost = 0;
+        std::vector<dcu_profile_window> rec; std::vector<std::vector<uint32_t>> sels; std::vector<dcu_overlap> ov;
+        for (int64_t b0 = minaread; b0 < lastop; b0 += (int64_t)std::max<uint64_t>(batchreads, 1)) {
+          const int64_t b1 = std::min<int64_t>(b0 + (int64_t)std::max<uint64_t>(batchreads, 1), lastop), nr = b1 - b0;
+          sels.assign((size_t)nr, {});
+#pragma omp parallel for schedule(dynamic, 8) num_threads(nthreads)
+          for (int64_t r = 0; r < nr; ++r) select_overlaps_profile(las, (uint64_t)(b0 + r), read_limit(db.rlen[b0 + r], maxinput, vard, avglen), sels[r]);
+          ov.clear();
+          for (auto& sel : sels)
+            for (auto i : sel) { const Overlap& o = las.ovl[i]; dcu_overlap x; memset(&x, 0, sizeof(x)); x.abpos = o.abpos; x.aepos = o.aepos; x.bbpos = o.bbpos; x.bepos = o.bepos; x.flags = o.flags; x.aread = o.aread; x.bread = o.bread; x.diffs = o.diffs; x.tlen = o.tlen; x.trace_off = o.trace_off; ov.push_back(x); }
+          uint64_t nrec = 0, hostw = 0;
+          rc = dcu_profile(ctx, ov.data(), ov.size(), las.trace.data(), las.trace.size(), las.tspace, db.boff.data(), db.rlen.data(), db.rlen.size(), maxalign, &nrec);
+          rec.resize(nrec);
+          if (!rc) rc = dcu_get_profile(ctx, rec.data());
+          if (rc) { fprintf(stderr, "[E] dcu_profile: %s: %s\n", dcu_strerror(rc), dcu_last_error(ctx)); return EXIT_FAILURE; }
+          dcu_last_profile_stats(ctx, &hostw); tothost += hostw;
+          for (const dcu_profile_window& r : rec) if (r.status == DCU_PROF_OK) vals.push_back(deep_value(r.cnt));
+          fprintf(stderr, "[V] reads [%ld,%ld) profile windows %lu\n", (long)b0, (long)b1, (unsigned long)nrec);
+        }
+        if (tothost) fprintf(stderr, "[V] %lu profile windows exceeded the GPU kernel's capacities and ran on the host\n", (unsigned long)tothost);
+        dcu_destroy(ctx);
+      }
+      const std::string text = deep_profile_text(vals);
+      fwrite(text.data(), 1, text.size(), stdout);
+      fflush(stdout);
+      lap("deep profile done");
+      return EXIT_SUCCESS;
+    }
     fprintf(stderr, "[V] minfilterfreq=%d maxfilterfreq=%d\n", prm.min_ff, prm.max_ff);
     // error profile: <las>.eprof or -E, in the reference's binary layout (eprof.hpp); estimated from the first <= 1024 A-reads when the
     // file does not exist, or is older than the .las and --keepeprof is off (reference src/daccord.cpp:1652-1880; keepeprof defaults to 1, :1303)

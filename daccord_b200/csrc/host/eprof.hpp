@@ -24,6 +24,7 @@
 #include "synth.hpp"
 #include "align.hpp"
 #include "pile.hpp"
+#include "../profile_core.cuh"
 
 namespace dhost {
 
@@ -235,14 +236,60 @@ inline void select_overlaps_profile(const LasData& L, uint64_t aread, uint64_t m
   std::stable_sort(sel.begin(), sel.end(), [&](uint32_t x, uint32_t y) { return L.ovl[x].abpos < L.ovl[y].abpos; });
 }
 
+// one window of the estimator (dcu_profile_window's layout): status DCU_PROF_* (profile_core.cuh ST_*), cnt = step counts of an OK window
+struct ProfileWindow { uint32_t aread, astart, status, reserved; uint32_t cnt[4]; };
+
+// runs a pile through profile_core.cuh's prof_window, the function the GPU profile kernel runs: with the kernel's capacities, and
+// when the window is beyond them (ST_HOST) once more with scratch sized to the window, as the library finishes such windows
+struct CoreEval {
+  std::vector<uint8_t> dev, own; std::vector<int32_t> dp;
+  uint64_t host_windows = 0;
+  int run(const std::vector<Seq>& pile, uint64_t g64[4]) {
+    using namespace dprof;
+    const uint32_t n = (uint32_t)pile.size();
+    uint32_t tot = 0, ml = 0; for (const Seq& s : pile) { tot += s.n; ml = std::max(ml, s.n); }
+    if (dev.empty()) dev.assign(scratch_bytes(PROF_MAXS, PROF_MAXB, PROF_HSZ, PROF_MAXLEN) + 16, 0);
+    uint32_t g[4] = {0, 0, 0, 0};
+    int st = ST_HOST;
+    if (n < 3 || (n <= PROF_MAXS && tot <= PROF_MAXB && ml <= PROF_MAXLEN)) {
+      Scratch S = scratch_at(align16(dev), PROF_MAXS, PROF_MAXB, PROF_HSZ, PROF_MAXLEN);
+      load(pile, S);
+      st = prof_window(n, S, g);
+    }
+    if (st == ST_HOST) {
+      ++host_windows;
+      uint32_t hsz = 16; while (hsz < 2 * tot + 2) hsz <<= 1;
+      own.assign(scratch_bytes(n, tot, hsz, ml) + 16, 0);
+      Scratch S = scratch_at(align16(own), n, tot, hsz, ml);
+      load(pile, S);
+      st = prof_window(n, S, g);
+      if (st == ST_HOST) {
+        dp.resize((size_t)(ml + 1) * (tot + 9)); S.dp = dp.data(); S.dp_cap = dp.size();
+        st = prof_window(n, S, g);
+      }
+      if (st == ST_HOST) throw std::runtime_error("profile window beyond its own scratch");
+    }
+    for (int i = 0; i < 4; ++i) g64[i] = g[i];
+    return st;
+  }
+ private:
+  static uint8_t* align16(std::vector<uint8_t>& v) { return (uint8_t*)(((uintptr_t)v.data() + 15) & ~(uintptr_t)15); }
+  static void load(const std::vector<Seq>& pile, const dprof::Scratch& S) {
+    uint32_t o = 0;
+    for (size_t i = 0; i < pile.size(); ++i) { S.soff[i] = o; memcpy(S.bases + o, pile[i].p, pile[i].n); o += pile[i].n; }
+    S.soff[pile.size()] = o;
+  }
+};
+
 class ProfileEstimator {
  public:
   enum { EW = 40, EA = 5 };                   // src/daccord.cpp:1279-1280
   ProfileEstimator(const PackedDB& rdb, const LasData& rL, uint64_t rmaxalign, uint64_t rmaxinput, uint64_t rvard = 0, uint64_t ravglen = 0)
       : db(rdb), L(rL), maxalign(rmaxalign), maxinput(rmaxinput), vard(rvard), avglen(ravglen), RP(rdb, rL, PileParams()) {}
 
-  // one A-read: adds to C, returns the mean error rate of its consensus windows (0 if none)
-  double read(uint64_t aread, ProfileCounts& C) {
+  // one A-read: adds to C, returns the mean error rate of its consensus windows (0 if none).  recs: if given, one record per window
+  // with a non-empty pile is appended; core: if given, the piles are evaluated by profile_core.cuh (CoreEval) instead of evaluate()
+  double read(uint64_t aread, ProfileCounts& C, std::vector<ProfileWindow>* recs = nullptr, CoreEval* core = nullptr) {
     select_overlaps_profile(L, aread, read_limit(db.rlen[aread], maxinput, vard, avglen), sel);
     const size_t nintv = sel.size();
     if (!nintv) return 0.0;
@@ -282,14 +329,17 @@ class ProfileEstimator {
         const size_t n0 = (size_t)(astart - o.abpos);
         pile.push_back(Seq{bseq[kv.second].data() + o.bbpos + m[n0], m[n0 + EW] - m[n0]});
       }
-      if (pile.size() < 3) continue;
-      bool rep = false;
-      for (const Seq& s : pile) if (repeats_kmer(s, TrivialConsensus::K - 1, tmp)) { rep = true; break; }
-      if (rep) { C.unusable++; continue; }
-      C.usable++;
-      if (!TC.run(pile, cons)) continue;
       uint64_t g[4] = {0, 0, 0, 0};
-      for (const Seq& s : pile) RP.TA.align_count(cons.data(), (int)cons.size(), s.p, (int)s.n, g);
+      const int st = core ? core->run(pile, g) : evaluate(g);
+      if (recs) {
+        ProfileWindow r; r.aread = (uint32_t)aread; r.astart = (uint32_t)astart; r.status = (uint32_t)st; r.reserved = 0;
+        for (int i = 0; i < 4; ++i) r.cnt[i] = (uint32_t)g[i];
+        recs->push_back(r);
+      }
+      if (st == dprof::ST_SKIPPED) continue;
+      if (st == dprof::ST_REPEAT) { C.unusable++; continue; }
+      C.usable++;
+      if (st != dprof::ST_OK) continue;
       for (int i = 0; i < 4; ++i) C.cnt[i] += g[i];
       esum += (double)(g[1] + g[2] + g[3]) / (double)(g[0] + g[1] + g[2] + g[3]);
       ++ecnt;
@@ -298,6 +348,14 @@ class ProfileEstimator {
   }
 
  private:
+  // the pile in `pile`: fewer than 3 sequences, a repeated 7-mer, no trivial consensus, or the step counts of the alignments to it
+  int evaluate(uint64_t g[4]) {
+    if (pile.size() < 3) return dprof::ST_SKIPPED;
+    for (const Seq& s : pile) if (repeats_kmer(s, TrivialConsensus::K - 1, tmp)) return dprof::ST_REPEAT;
+    if (!TC.run(pile, cons)) return dprof::ST_NO_CONSENSUS;
+    for (const Seq& s : pile) RP.TA.align_count(cons.data(), (int)cons.size(), s.p, (int)s.n, g);
+    return dprof::ST_OK;
+  }
   const PackedDB& db; const LasData& L; uint64_t maxalign, maxinput, vard, avglen;
   ReadPiler RP;                                // for its tile aligner and trace reconstruction
   TrivialConsensus TC;
@@ -335,6 +393,53 @@ inline ProfileCounts estimate_profile(const PackedDB& db, const LasData& L, int6
     R.edif = std::sqrt(d / (double)n);
   }
   return R;
+}
+
+// the windows of A-reads [lo, hi) in read order (no cap on the read count); core: evaluate the piles with profile_core.cuh (CoreEval),
+// *host_windows = the windows beyond the GPU kernel's capacities
+inline std::vector<ProfileWindow> profile_windows(const PackedDB& db, const LasData& L, int64_t lo, int64_t hi, uint64_t maxalign, uint64_t maxinput, int nthreads,
+                                                  uint64_t vard, uint64_t avglen, bool core, uint64_t* host_windows) {
+  const int64_t nr = std::max<int64_t>(hi - lo, 0);
+  std::vector<std::vector<ProfileWindow>> per(nr); uint64_t hw = 0;
+  if (nthreads < 1) nthreads = 1;
+#pragma omp parallel num_threads(nthreads) reduction(+ : hw)
+  {
+    ProfileEstimator PE(db, L, maxalign, maxinput, vard, avglen);
+    CoreEval CE; ProfileCounts C;
+#pragma omp for schedule(dynamic, 1)
+    for (int64_t i = 0; i < nr; ++i) {
+      if (L.aidx[lo + i] == L.aidx[lo + i + 1]) continue;
+      PE.read((uint64_t)(lo + i), C, &per[i], core ? &CE : nullptr);
+    }
+    hw += CE.host_windows;
+  }
+  std::vector<ProfileWindow> R;
+  for (auto& v : per) R.insert(R.end(), v.begin(), v.end());
+  if (host_windows) *host_windows = hw;
+  return R;
+}
+
+// --deepprofileonly (reference src/daccord.cpp:1442-1650, :945-955): every consensus window's error rate e = (mis + ins + del) / (all
+// steps) as v = min(uint64(4294967295 e + 0.5), 2^32 - 1); per distinct v in ascending order one line "[deep]\t{v / 4294967295}\t{share of
+// windows with a value <= v}", both numbers as %g (the reference's default ostream formatting)
+inline std::string deep_profile_text(std::vector<uint32_t>& v) {
+  std::sort(v.begin(), v.end());
+  std::string out; char buf[96];
+  const double dcnt = (double)v.size();
+  uint64_t s = 0;
+  for (size_t l = 0; l < v.size();) {
+    size_t h = l; while (h < v.size() && v[h] == v[l]) ++h;
+    s += h - l;
+    snprintf(buf, sizeof buf, "[deep]\t%g\t%g\n", (double)v[l] / 4294967295.0, (double)s / dcnt);
+    out += buf; l = h;
+  }
+  return out;
+}
+inline uint32_t deep_value(const uint32_t cnt[4]) {
+  const uint64_t e = (uint64_t)cnt[1] + cnt[2] + cnt[3], all = e + cnt[0];
+  const double rate = (double)e / (double)all;
+  const uint64_t v = (uint64_t)(4294967295.0 * rate + 0.5);
+  return (uint32_t)std::min<uint64_t>(v, 4294967295ull);
 }
 
 }  // namespace dhost

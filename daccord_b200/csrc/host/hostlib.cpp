@@ -179,14 +179,16 @@ void dh_batch_destroy(dh_batch* b) { delete b; }
 // the overlaps daccord would hand to HandleContext for A-reads [first,last): top-D selection, ordered by abpos
 // (reference src/daccord.cpp:2112-2288), in the dcu_overlap form of the C ABI.  Buffers are malloc'ed (dh_free).
 struct dh_ovlset { std::vector<dcu_overlap> ovl; };
-dh_ovlset* dh_select_overlaps_vard(dh_data* d, uint64_t first_read, uint64_t last_read, uint64_t maxinput, uint64_t vard) {
+// profile != 0: the error-profile estimator's selection (the maxinput LOWEST-scoring overlaps, select_overlaps_profile), what dcu_profile takes
+dh_ovlset* dh_select_overlaps_mode(dh_data* d, uint64_t first_read, uint64_t last_read, uint64_t maxinput, uint64_t vard, int profile) {
   std::unique_ptr<dh_ovlset> S(new dh_ovlset());
   uint64_t avglen;
   if (!vard_avglen(d, vard, avglen)) return nullptr;
   if (last_read > d->nA) last_read = d->nA;
   std::vector<uint32_t> sel;
   for (uint64_t r = first_read; r < last_read; ++r) {
-    select_overlaps(d->las, r, read_limit(d->db.rlen[r], maxinput, vard, avglen), sel);
+    if (profile) select_overlaps_profile(d->las, r, read_limit(d->db.rlen[r], maxinput, vard, avglen), sel);
+    else select_overlaps(d->las, r, read_limit(d->db.rlen[r], maxinput, vard, avglen), sel);
     for (auto i : sel) {
       const Overlap& o = d->las.ovl[i];
       dcu_overlap x; memset(&x, 0, sizeof(x));
@@ -196,6 +198,9 @@ dh_ovlset* dh_select_overlaps_vard(dh_data* d, uint64_t first_read, uint64_t las
     }
   }
   return S.release();
+}
+dh_ovlset* dh_select_overlaps_vard(dh_data* d, uint64_t first_read, uint64_t last_read, uint64_t maxinput, uint64_t vard) {
+  return dh_select_overlaps_mode(d, first_read, last_read, maxinput, vard, 0);
 }
 dh_ovlset* dh_select_overlaps(dh_data* d, uint64_t first_read, uint64_t last_read, uint64_t maxinput) { return dh_select_overlaps_vard(d, first_read, last_read, maxinput, 0); }
 const dcu_overlap* dh_ovlset_data(dh_ovlset* s, uint64_t* n) { *n = s->ovl.size(); return s->ovl.data(); }
@@ -264,6 +269,23 @@ int dh_estimate_profile_vard(dh_data* d, int64_t first_read, int64_t last_read, 
     if (dout2) { dout2[0] = C.eavg; dout2[1] = C.edif; }
     return 0;
   } catch (std::exception& e) { d->err = e.what(); return 1; }
+}
+// the estimator's windows of A-reads [first_read, last_read) (no cap on the count): one record per window with a non-empty pile, in read
+// and window order (dcu_profile_window layout); core != 0: piles evaluated by profile_core.cuh (the GPU kernel's function, with its
+// capacities, then sized to the window), *host_windows = windows beyond the kernel's capacities.  Returns a malloc'ed array (dh_free)
+ProfileWindow* dh_profile_windows(dh_data* d, int64_t first_read, int64_t last_read, uint64_t maxalign, uint64_t maxinput, uint64_t vard, int core, int nthreads,
+                                  uint64_t* n, uint64_t* host_windows) {
+  try {
+    uint64_t avglen;
+    if (!vard_avglen(d, vard, avglen)) return nullptr;
+    if (first_read < 0) first_read = 0;
+    if (last_read < 0 || last_read > (int64_t)d->nA) last_read = (int64_t)d->nA;
+    std::vector<ProfileWindow> R = profile_windows(d->db, d->las, first_read, last_read, maxalign, maxinput, nthreads, vard, avglen, core != 0, host_windows);
+    ProfileWindow* out = (ProfileWindow*)malloc(std::max<size_t>(R.size(), 1) * sizeof(ProfileWindow));
+    if (!R.empty()) memcpy(out, R.data(), R.size() * sizeof(ProfileWindow));
+    *n = R.size();
+    return out;
+  } catch (std::exception& e) { d->err = e.what(); return nullptr; }
 }
 int dh_estimate_profile(dh_data* d, int64_t first_read, int64_t last_read, uint64_t maxalign, uint64_t maxinput, int nthreads, uint64_t* out7, double* dout2) {
   return dh_estimate_profile_vard(d, first_read, last_read, maxalign, maxinput, 0, nthreads, out7, dout2);

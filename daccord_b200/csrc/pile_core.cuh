@@ -8,7 +8,8 @@
 //                      vectors and a bit-vector traceback (rule: diagonal, DEL, INS); records the B offset reached
 //                      after every A position that a window boundary can fall on
 //   pile_order       : per A-read, its overlaps in pile order (escore<<32)|z
-//   pile_window      : per window, the pile (a pure function of the read's overlaps, see below) and its slices
+//   pile_window      : per window, the pile (a pure function of the read's overlaps, see below) and its slices; pile_window_m<true>
+//                      builds the piles of the error-profile estimator instead (profile_core.cuh evaluates them)
 // Requirement of this path (checked by the host, which otherwise uses the host piler): A tile <= 128 (tspace <= 128).
 // The same source is compiled for the host (tests/emu, -DDCU_EMU) to check it against the host piler without a GPU.
 #pragma once
@@ -177,16 +178,21 @@ PILE_FN void pile_order(const ReadInfo& R, const Ovl* ovl, double minerate, doub
 // win == nullptr: returns the number of slices (0: empty pile, no window is emitted).  Otherwise writes the window
 // descriptor to *win and its slices to sl[0 .. n) with slice_begin = sl_index; returns n, or -1 if a slice length does not fit the descriptor (16 bit).  Slices longer than 255 bases are
 // written as they are: the window kernel ends such a window as DCU_WIN_OVERFLOW (8-bit instance positions), the batch goes on.
-PILE_FN int pile_window(const ReadInfo& R, uint32_t y, const Ovl* ovl, const Params& P, const uint32_t* bm, const uint64_t* read_boff, const uint32_t* read_len,
-                        const unsigned long long* keys, uint32_t aread, Win* win, Sl* sl, uint32_t sl_index) {
+//
+// PROF (the error-profile estimator's piles, reference src/daccord.cpp:400-530): windows y * a for y < prof_win_count (no final window
+// at l - w), and an overlap is a member iff abpos <= astart && aepos > aend -- the estimator expires overlaps with <= (:481-485) where
+// the main loop uses <.  Pile order and the maxalign cap are the main loop's.
+template <bool PROF>
+PILE_FN int pile_window_m(const ReadInfo& R, uint32_t y, const Ovl* ovl, const Params& P, const uint32_t* bm, const uint64_t* read_boff, const uint32_t* read_len,
+                          const unsigned long long* keys, uint32_t aread, Win* win, Sl* sl, uint32_t sl_index) {
   const uint64_t nintv = R.ovl_end - R.ovl_begin;
   const uint64_t l = R.maxaepos;
-  const uint64_t astart = win_start(y, l, P.a, P.w), aend = astart + P.w;
+  const uint64_t astart = PROF ? (uint64_t)y * P.a : win_start(y, l, P.a, P.w), aend = astart + P.w;
   const uint32_t special0 = l >= P.w ? (uint32_t)(l - P.w) : 0, special1 = (uint32_t)l;
   uint64_t MAo = 0; int ns = 0;
   for (uint64_t t = 0; t < nintv; ++t) {                                            // members in pile order (:1984-2049)
     const Ovl& o = ovl[R.ovl_begin + (keys[t] & 0xFFFFFFFFull)];
-    if (!((int64_t)astart >= o.abpos && (uint64_t)o.aepos >= aend)) continue;
+    if (!((int64_t)astart >= o.abpos && (PROF ? (uint64_t)o.aepos > aend : (uint64_t)o.aepos >= aend))) continue;
     if (!MAo) { if (win) { sl[ns].gpos = (uint32_t)(read_boff[aread] * 4 + astart); sl[ns].len = (uint16_t)P.w; sl[ns].flags = 0; } ++ns; ++MAo; }
     if (MAo < P.maxalign) {
       if (win) {
@@ -203,5 +209,11 @@ PILE_FN int pile_window(const ReadInfo& R, uint32_t y, const Ovl* ovl, const Par
   if (MAo && win) { win->slice_begin = sl_index; win->slice_cnt = (uint16_t)(MAo > 65535 ? 65535 : MAo); win->reserved = 0; win->aread = aread; win->astart = (uint32_t)astart; }
   return ns;
 }
+PILE_FN int pile_window(const ReadInfo& R, uint32_t y, const Ovl* ovl, const Params& P, const uint32_t* bm, const uint64_t* read_boff, const uint32_t* read_len,
+                        const unsigned long long* keys, uint32_t aread, Win* win, Sl* sl, uint32_t sl_index) {
+  return pile_window_m<false>(R, y, ovl, P, bm, read_boff, read_len, keys, aread, win, sl, sl_index);
+}
+// windows of the error-profile estimator: y * a for y < (l + a - w) / a (reference src/daccord.cpp:408)
+PILE_HD uint64_t prof_win_count(uint64_t l, uint64_t a, uint64_t w) { return l + a >= w ? (l + a - w) / a : 0; }
 
 }  // namespace dpile

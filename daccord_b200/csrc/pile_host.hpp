@@ -17,7 +17,9 @@ struct Prep {
   std::string err;
 };
 
-inline bool prepare(const dcu_overlap* in, uint64_t novl, uint64_t ntrace, int32_t tspace, uint32_t w, uint32_t a, uint64_t nreads, const uint32_t* read_len, Prep& P) {
+// prof: candidate windows of the error-profile estimator (pile_window_m<true>) instead of the main loop's
+inline bool prepare(const dcu_overlap* in, uint64_t novl, uint64_t ntrace, int32_t tspace, uint32_t w, uint32_t a, uint64_t nreads, const uint32_t* read_len, Prep& P,
+                    bool prof = false) {
   if (tspace <= 0 || tspace > 128) { P.err = "tspace outside (0,128]"; return false; }
   if (a == 0) { P.err = "advance size 0"; return false; }
   P.ovl.resize(novl); P.reads.clear(); P.read_id.clear(); P.minerate.clear(); P.ediv.clear();
@@ -41,7 +43,7 @@ inline bool prepare(const dcu_overlap* in, uint64_t novl, uint64_t ntrace, int32
   }
   P.ntiles = toff; P.nbm = boff;
   P.ncand = 0;
-  for (auto& R : P.reads) { R.win_off = P.ncand; R.nwin = (uint32_t)win_count(R.maxaepos, a, w); P.ncand += R.nwin; }
+  for (auto& R : P.reads) { R.win_off = P.ncand; R.nwin = (uint32_t)(prof ? prof_win_count(R.maxaepos, a, w) : win_count(R.maxaepos, a, w)); P.ncand += R.nwin; }
   P.minerate.resize(P.reads.size()); P.ediv.resize(P.reads.size());
   for (size_t r = 0; r < P.reads.size(); ++r) {       // HandleContext.hpp:1780-1790
     double mx = 0.0, mn = 1.0;

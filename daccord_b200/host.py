@@ -19,7 +19,7 @@ def lib():
             raise DcuError("host library %s not built: run `python -m daccord_b200.build`" % HOST_LIB_PATH)
         L = C.CDLL(HOST_LIB_PATH)
         for f in ("dh_sim_create", "dh_sim_create_ex", "dh_sim_create_spread", "dh_data_load", "dh_data_load2", "dh_pile_vard", "dh_select_overlaps_vard", "dh_data_load_range", "dh_pile", "dh_vote", "dh_data_packed", "dh_batch_windows", "dh_batch_slices", "dh_batch_read_first",
-                  "dh_select_overlaps", "dh_ovlset_data", "dh_data_trace", "dh_data_boff", "dh_data_rlen", "dh_format_segments"):
+                  "dh_select_overlaps", "dh_select_overlaps_mode", "dh_profile_windows", "dh_ovlset_data", "dh_data_trace", "dh_data_boff", "dh_data_rlen", "dh_format_segments"):
             getattr(L, f).restype = C.c_void_p
         for f in ("dh_data_nreads", "dh_data_nall", "dh_data_novl", "dh_data_totlen"):
             getattr(L, f).restype = C.c_uint64
@@ -132,10 +132,28 @@ class Dataset:
         out["eavg"], out["edif"] = float(d[0]), float(d[1])
         return out
 
-    def overlaps(self, first=0, last=None, maxinput=5000, vard=0):
-        """selected overlaps of A-reads [first,last) in dcu_overlap form + the trace array + read offsets / lengths of all reads (numpy copies)"""
+    def profile_windows(self, first=0, top=None, maxalign=2**64 - 1, maxinput=5000, vard=0, core=False, nthreads=0):
+        """the error-profile estimator's windows of A-reads [first, top) (no cap on the count): one record per window with a non-empty pile,
+        in read and window order, as daccord_b200.PROFILE_WINDOW_DT (status 0 skipped, 1 repeat, 2 no consensus, 3 ok; cnt = matches,
+        mismatches, insertions, deletions).  core: piles evaluated by the GPU kernel's per-window function (profile_core.cuh) compiled for
+        the host.  Returns (records, windows beyond the kernel's capacities; 0 unless core)."""
+        from . import PROFILE_WINDOW_DT
+        n, hw = C.c_uint64(0), C.c_uint64(0)
+        top = -1 if top is None else top
+        p = lib().dh_profile_windows(self.h, C.c_int64(first), C.c_int64(top), C.c_uint64(maxalign), C.c_uint64(maxinput), C.c_uint64(vard),
+                                     C.c_int(1 if core else 0), C.c_int(nthreads or (os.cpu_count() or 1)), C.byref(n), C.byref(hw))
+        if not p:
+            raise DcuError(lib().dh_data_error(self.h).decode())
+        rec = np.frombuffer((C.c_uint8 * (n.value * PROFILE_WINDOW_DT.itemsize)).from_address(p), dtype=PROFILE_WINDOW_DT).copy() if n.value \
+            else np.zeros(0, PROFILE_WINDOW_DT)
+        lib().dh_free(C.c_void_p(p))
+        return rec, hw.value
+
+    def overlaps(self, first=0, last=None, maxinput=5000, vard=0, profile=False):
+        """selected overlaps of A-reads [first,last) in dcu_overlap form + the trace array + read offsets / lengths of all reads (numpy copies);
+        profile: the error-profile estimator's selection (the maxinput lowest-scoring overlaps), what Engine.profile takes"""
         last = self.nreads if last is None else last
-        h = lib().dh_select_overlaps_vard(self.h, C.c_uint64(first), C.c_uint64(last), C.c_uint64(maxinput), C.c_uint64(vard))
+        h = lib().dh_select_overlaps_mode(self.h, C.c_uint64(first), C.c_uint64(last), C.c_uint64(maxinput), C.c_uint64(vard), C.c_int(1 if profile else 0))
         if not h:
             raise DcuError(lib().dh_data_error(self.h).decode())
         n = C.c_uint64(0)

@@ -133,6 +133,27 @@ int dcu_vote(dcu_ctx* ctx, int producefull, uint64_t minlen, const uint64_t* rea
              uint64_t* nseg, uint64_t* nchars);
 /* segments (in A-read, position order) and the character buffer (nchars bytes) of the last dcu_vote */
 int dcu_get_corrected(dcu_ctx* ctx, dcu_segment* seg, char* chars);
+/* ---- error-profile windows on the GPU -------------------------------------------------------------------------------
+ * The per-window work of the reference's error-profile estimator (src/daccord.cpp:271-631, and :634-995 for --deepprofileonly):
+ * windows of 40 bases advancing by 5 (y * 5 for y < (maxaepos + 5 - 40) / 5, no final window at l - w), the pile of a window = the A
+ * window and the B slices of every overlap with abpos <= astart and aepos > aend, in the main loop's pile order, at most maxalign
+ * sequences (-d).  Input: the overlaps selected by the estimator's rule (the -D / --vard LOWEST-scoring ones, ordered by abpos), in the
+ * form and order of dcu_pile, with tspace <= 128.  Output: one record per window with a non-empty pile, in (aread, astart) order:
+ *   DCU_PROF_SKIPPED       fewer than 3 sequences
+ *   DCU_PROF_REPEAT        some sequence repeats a 7-mer (not usable)
+ *   DCU_PROF_NO_CONSENSUS  usable, but the k = 8 graph has no trivial consensus
+ *   DCU_PROF_OK            cnt = matches, mismatches, insertions, deletions of every sequence aligned to the consensus
+ * Windows beyond the kernel's per-thread capacities (more than 128 sequences or 4096 bases, a sequence longer than 255 bases, a consensus
+ * longer than 128 bases) are finished on the host by the same per-window function; dcu_last_profile_stats counts them.  The call replaces
+ * the context's resident batch (run dcu_pile / dcu_upload again before dcu_launch). */
+enum { DCU_PROF_SKIPPED = 0, DCU_PROF_REPEAT = 1, DCU_PROF_NO_CONSENSUS = 2, DCU_PROF_OK = 3 };
+typedef struct dcu_profile_window { uint32_t aread, astart, status, reserved; uint32_t cnt[4]; } dcu_profile_window;
+int dcu_profile(dcu_ctx* ctx, const dcu_overlap* ovl, uint64_t novl, const uint16_t* trace, uint64_t ntrace, int32_t tspace,
+                const uint64_t* read_boff, const uint32_t* read_len, uint64_t nreads, uint64_t maxalign, uint64_t* nrec);
+/* the records of the last dcu_profile (nrec entries) */
+int dcu_get_profile(dcu_ctx* ctx, dcu_profile_window* rec);
+/* windows of the last dcu_profile that were finished on the host */
+int dcu_last_profile_stats(dcu_ctx* ctx, uint64_t* host_windows);
 /* statistics of the last launch: kernels launched, windows that needed the large-workspace pass */
 int dcu_last_stats(dcu_ctx* ctx, uint64_t* launches, uint64_t* hard_windows);
 /* more statistics of the last launch: windows the first pass handed to the plain HBM passes, windows beyond every capacity
