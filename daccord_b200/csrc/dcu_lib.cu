@@ -547,6 +547,17 @@ const char* dcu_strerror(int code) {
 }
 const char* dcu_last_error(dcu_ctx* ctx) { return ctx ? ctx->err.c_str() : "null ctx"; }
 
+int dcu_device_count(int* n) {
+  if (!n) return DCU_ERR_PARAM;
+  *n = 0;
+  int c = 0;
+  const cudaError_t e = cudaGetDeviceCount(&c);
+  if (e == cudaErrorNoDevice || e == cudaErrorInsufficientDriver) { cudaGetLastError(); return DCU_OK; }     // no device, or no driver: none
+  if (e != cudaSuccess) { cudaGetLastError(); return DCU_ERR_CUDA; }
+  *n = c;
+  return DCU_OK;
+}
+
 int dcu_create(const dcu_params* p, int device, dcu_ctx** out) {
   if (!p || !out) return DCU_ERR_PARAM;
   *out = nullptr;

@@ -3,6 +3,7 @@
 // with the per-window consensus running on an H100 through the C ABI in include/daccord_b200.h.
 // Host side (this file + pile.hpp / vote.hpp): LAS + Dazzler-DB input, overlap selection, trace reconstruction,
 // window/slice extraction, pile vote, FastA on stdout, progress on stderr.
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -66,6 +67,43 @@ static bool parse_args(int argc, char** argv, Args& A) {
 }
 static bool parse_pair(const std::string& s, int64_t& a, int64_t& b) { return sscanf(s.c_str(), "%ld,%ld", &a, &b) == 2; }
 
+static_assert(sizeof(ProfileWindow) == sizeof(dcu_profile_window) && offsetof(ProfileWindow, cnt) == offsetof(dcu_profile_window, cnt), "one record layout");
+
+// the error-profile estimator's windows of A-reads [lo, hi) on the GPU, in (aread, astart) order: the estimator's overlap selection
+// (select_overlaps_profile) per batch of `batchreads` reads, dcu_profile on a context of its own, destroyed before returning so that its
+// per-thread scratch is free again.  *host_windows = windows dcu_profile finished on the host.  false: an error (printed)
+static bool gpu_profile_windows(const PackedDB& db, const LasData& las, int64_t lo, int64_t hi, uint64_t maxalign, uint64_t maxinput, uint64_t vard,
+                                uint64_t avglen, uint64_t batchreads, int device, int nthreads, std::vector<ProfileWindow>& out, uint64_t* host_windows) {
+  out.clear(); *host_windows = 0;
+  dcu_params pp; memset(&pp, 0, sizeof(pp));
+  pp.w = 40; pp.k_lo = pp.k_hi = 8; pp.min_cov = 3; pp.min_ff = 0; pp.max_ff = 2; pp.max_err = UINT64_MAX; pp.p_i = 0.09; pp.p_d = 0.045; pp.est_cor = 0.85;
+  dcu_ctx* ctx = nullptr;
+  int rc = dcu_create(&pp, device, &ctx);
+  if (!rc) rc = dcu_set_reads(ctx, db.bytes.data(), db.bytes.size());
+  if (rc) { fprintf(stderr, "[E] dcu_create / dcu_set_reads: %s %s\n", dcu_strerror(rc), ctx ? dcu_last_error(ctx) : ""); dcu_destroy(ctx); return false; }
+  const int64_t step = (int64_t)std::max<uint64_t>(batchreads, 1);
+  std::vector<std::vector<uint32_t>> sels; std::vector<dcu_overlap> ov;
+  for (int64_t b0 = lo; b0 < hi; b0 += step) {
+    const int64_t b1 = std::min<int64_t>(b0 + step, hi), nr = b1 - b0;
+    sels.assign((size_t)nr, {});
+#pragma omp parallel for schedule(dynamic, 8) num_threads(nthreads)
+    for (int64_t r = 0; r < nr; ++r) select_overlaps_profile(las, (uint64_t)(b0 + r), read_limit(db.rlen[b0 + r], maxinput, vard, avglen), sels[r]);
+    ov.clear();
+    for (auto& sel : sels)
+      for (auto i : sel) { const Overlap& o = las.ovl[i]; dcu_overlap x; memset(&x, 0, sizeof(x)); x.abpos = o.abpos; x.aepos = o.aepos; x.bbpos = o.bbpos; x.bepos = o.bepos; x.flags = o.flags; x.aread = o.aread; x.bread = o.bread; x.diffs = o.diffs; x.tlen = o.tlen; x.trace_off = o.trace_off; ov.push_back(x); }
+    uint64_t nrec = 0, hostw = 0;
+    rc = dcu_profile(ctx, ov.data(), ov.size(), las.trace.data(), las.trace.size(), las.tspace, db.boff.data(), db.rlen.data(), db.rlen.size(), maxalign, &nrec);
+    const size_t n0 = out.size();
+    out.resize(n0 + nrec);
+    if (!rc) rc = dcu_get_profile(ctx, reinterpret_cast<dcu_profile_window*>(out.data() + n0));
+    if (rc) { fprintf(stderr, "[E] dcu_profile: %s: %s\n", dcu_strerror(rc), dcu_last_error(ctx)); dcu_destroy(ctx); return false; }
+    dcu_last_profile_stats(ctx, &hostw); *host_windows += hostw;
+    fprintf(stderr, "[V] reads [%ld,%ld) profile windows %lu\n", (long)b0, (long)b1, (unsigned long)nrec);
+  }
+  dcu_destroy(ctx);
+  return true;
+}
+
 int main(int argc, char** argv) {
   Args A;
   if (!parse_args(argc, argv, A)) return EXIT_FAILURE;
@@ -126,46 +164,27 @@ int main(int argc, char** argv) {
     }
     fprintf(stderr, "done (%zu of %ld overlaps).\n", las.ovl.size(), (long)lidx.novl);
     lap("inputs loaded");
+    // error profile: <las>.eprof or -E, in the reference's binary layout (eprof.hpp); estimated from the first <= 1024 A-reads when the
+    // file does not exist, or is older than the .las and --keepeprof is off (reference src/daccord.cpp:1652-1880; keepeprof defaults to 1, :1303)
+    const std::string eproffn = A.opt.count("E") ? A.opt["E"] : lasfn + ".eprof";
+    const bool estimate = !deep && eprof_is_stale(eproffn, lasfn, getu("keepeprof", 1) != 0);
+    // the error-profile estimator's windows (--deepprofileonly, and the estimate) run on the GPU (gpu_profile_windows) unless
+    // DACCORD_HOST_PROFILE is set or the trace tiles are longer than the GPU piler aligns; then on the host (eprof.hpp)
+    const bool host_prof_env = getenv("DACCORD_HOST_PROFILE") != nullptr;
+    if (!host_prof_env && las.tspace > 128 && (deep || estimate))
+      fprintf(stderr, "[W] the profile windows run on the host for this input (the GPU piler aligns trace tiles of at most 128 A bases; here tspace=%d)\n", las.tspace);
+    const bool host_prof = host_prof_env || las.tspace > 128;
     if (deep) {
       // --deepprofileonly (reference src/daccord.cpp:1442-1650): the error-profile estimator's windows over A-reads [minaread, lastop), the
       // error rate of every window with a consensus, printed as its cumulative distribution; no error profile is read or written.
-      // The windows run on the GPU (dcu_profile) in batches of --batchreads reads; DACCORD_HOST_PROFILE=1, or trace tiles longer than the GPU
-      // piler takes, run them on the host (eprof.hpp)
       std::vector<uint32_t> vals;
-      const bool host_prof = getenv("DACCORD_HOST_PROFILE") != nullptr;
-      if (host_prof || las.tspace > 128) {
-        if (!host_prof) fprintf(stderr, "[W] the profile windows run on the host for this input (the GPU piler aligns trace tiles of at most 128 A bases; here tspace=%d)\n", las.tspace);
-        for (const ProfileWindow& r : profile_windows(db, las, minaread, lastop, maxalign, maxinput, nthreads, vard, avglen, false, nullptr))
-          if (r.status == DCU_PROF_OK) vals.push_back(deep_value(r.cnt));
-      } else {
-        dcu_params pp; memset(&pp, 0, sizeof(pp));
-        pp.w = 40; pp.k_lo = pp.k_hi = 8; pp.min_cov = 3; pp.min_ff = 0; pp.max_ff = 2; pp.max_err = UINT64_MAX; pp.p_i = 0.09; pp.p_d = 0.045; pp.est_cor = 0.85;
-        dcu_ctx* ctx = nullptr;
-        int rc = dcu_create(&pp, device, &ctx);
-        if (!rc) rc = dcu_set_reads(ctx, db.bytes.data(), db.bytes.size());
-        if (rc) { fprintf(stderr, "[E] dcu_create / dcu_set_reads: %s %s\n", dcu_strerror(rc), ctx ? dcu_last_error(ctx) : ""); return EXIT_FAILURE; }
-        uint64_t tothost = 0;
-        std::vector<dcu_profile_window> rec; std::vector<std::vector<uint32_t>> sels; std::vector<dcu_overlap> ov;
-        for (int64_t b0 = minaread; b0 < lastop; b0 += (int64_t)std::max<uint64_t>(batchreads, 1)) {
-          const int64_t b1 = std::min<int64_t>(b0 + (int64_t)std::max<uint64_t>(batchreads, 1), lastop), nr = b1 - b0;
-          sels.assign((size_t)nr, {});
-#pragma omp parallel for schedule(dynamic, 8) num_threads(nthreads)
-          for (int64_t r = 0; r < nr; ++r) select_overlaps_profile(las, (uint64_t)(b0 + r), read_limit(db.rlen[b0 + r], maxinput, vard, avglen), sels[r]);
-          ov.clear();
-          for (auto& sel : sels)
-            for (auto i : sel) { const Overlap& o = las.ovl[i]; dcu_overlap x; memset(&x, 0, sizeof(x)); x.abpos = o.abpos; x.aepos = o.aepos; x.bbpos = o.bbpos; x.bepos = o.bepos; x.flags = o.flags; x.aread = o.aread; x.bread = o.bread; x.diffs = o.diffs; x.tlen = o.tlen; x.trace_off = o.trace_off; ov.push_back(x); }
-          uint64_t nrec = 0, hostw = 0;
-          rc = dcu_profile(ctx, ov.data(), ov.size(), las.trace.data(), las.trace.size(), las.tspace, db.boff.data(), db.rlen.data(), db.rlen.size(), maxalign, &nrec);
-          rec.resize(nrec);
-          if (!rc) rc = dcu_get_profile(ctx, rec.data());
-          if (rc) { fprintf(stderr, "[E] dcu_profile: %s: %s\n", dcu_strerror(rc), dcu_last_error(ctx)); return EXIT_FAILURE; }
-          dcu_last_profile_stats(ctx, &hostw); tothost += hostw;
-          for (const dcu_profile_window& r : rec) if (r.status == DCU_PROF_OK) vals.push_back(deep_value(r.cnt));
-          fprintf(stderr, "[V] reads [%ld,%ld) profile windows %lu\n", (long)b0, (long)b1, (unsigned long)nrec);
-        }
+      std::vector<ProfileWindow> rec; uint64_t tothost = 0;
+      if (host_prof) rec = profile_windows(db, las, minaread, lastop, maxalign, maxinput, nthreads, vard, avglen, false, nullptr);
+      else {
+        if (!gpu_profile_windows(db, las, minaread, lastop, maxalign, maxinput, vard, avglen, batchreads, device, nthreads, rec, &tothost)) return EXIT_FAILURE;
         if (tothost) fprintf(stderr, "[V] %lu profile windows exceeded the GPU kernel's capacities and ran on the host\n", (unsigned long)tothost);
-        dcu_destroy(ctx);
       }
+      for (const ProfileWindow& r : rec) if (r.status == DCU_PROF_OK) vals.push_back(deep_value(r.cnt));
       const std::string text = deep_profile_text(vals);
       fwrite(text.data(), 1, text.size(), stdout);
       fflush(stdout);
@@ -173,13 +192,28 @@ int main(int argc, char** argv) {
       return EXIT_SUCCESS;
     }
     fprintf(stderr, "[V] minfilterfreq=%d maxfilterfreq=%d\n", prm.min_ff, prm.max_ff);
-    // error profile: <las>.eprof or -E, in the reference's binary layout (eprof.hpp); estimated from the first <= 1024 A-reads when the
-    // file does not exist, or is older than the .las and --keepeprof is off (reference src/daccord.cpp:1652-1880; keepeprof defaults to 1, :1303)
-    std::string eproffn = A.opt.count("E") ? A.opt["E"] : lasfn + ".eprof";
-    const bool keepeprof = getu("keepeprof", 1) != 0;
     uint64_t ecnt[4] = {0, 0, 0, 0};
-    if (eprof_is_stale(eproffn, lasfn, keepeprof)) {
-      ProfileCounts PC = estimate_profile(db, las, minaread, toparead, maxalign, maxinput, nthreads, vard, avglen);
+    if (estimate) {
+      // on the GPU as above, and on the host also when this process sees no CUDA device.  Either way the windows' records are summed by
+      // profile_counts, so both give the same file; the profile context is gone before the main contexts are created
+      const int64_t etop = std::min<int64_t>(toparead, minaread + 1024);
+      int ndev = 0;
+      if (!host_prof) {
+        const int rc = dcu_device_count(&ndev);
+        if (rc) { fprintf(stderr, "[E] dcu_device_count: %s\n", dcu_strerror(rc)); return EXIT_FAILURE; }
+      }
+      ProfileCounts PC;
+      if (host_prof || ndev == 0) {
+        fprintf(stderr, "[V] error profile: windows of reads [%ld,%ld) on the host (%s)\n", (long)minaread, (long)std::max(etop, minaread),
+                host_prof_env ? "DACCORD_HOST_PROFILE" : host_prof ? "tspace > 128" : "no CUDA device");
+        PC = estimate_profile(db, las, minaread, toparead, maxalign, maxinput, nthreads, vard, avglen);
+      } else {
+        std::vector<ProfileWindow> rec; uint64_t hostw = 0;
+        if (!gpu_profile_windows(db, las, minaread, etop, maxalign, maxinput, vard, avglen, batchreads, device, nthreads, rec, &hostw)) return EXIT_FAILURE;
+        fprintf(stderr, "[V] error profile: windows of reads [%ld,%ld) on the GPU (device %d), %lu windows, %lu of them finished on the host\n", (long)minaread,
+                (long)std::max(etop, minaread), device, (unsigned long)rec.size(), (unsigned long)hostw);
+        PC = profile_counts(rec.data(), rec.size());
+      }
       fprintf(stderr, "usable=%lu unusable=%lu eavg=%g edif=%g\n", (unsigned long)PC.usable, (unsigned long)PC.unusable, PC.eavg, PC.edif);
       write_eprof(eproffn, PC.cnt, PC.eavg, PC.edif);
     }

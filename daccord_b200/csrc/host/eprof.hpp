@@ -7,7 +7,8 @@
 // first k-mer to the most frequent last k-mer; every pile sequence is aligned to it and the step counts (match, mismatch,
 // insertion, deletion) summed over all windows are the profile the OffsetLikely / KmerLimit tables are built from.
 //
-// This runs once per input on a bounded sample, so it stays on the host (the product's hot path is the main loop).
+// The daccord CLI runs these windows on the GPU (dcu_profile) when it can and sums the records with profile_counts below; this host
+// estimator is the fallback (no device, tspace > 128, DACCORD_HOST_PROFILE) and the reference the GPU records are tested against.
 // Own formulation: dense 4^8 count tables and explicit unitig vectors instead of the reference's sorted node arrays.
 #pragma once
 #include <cstdint>
@@ -287,12 +288,12 @@ class ProfileEstimator {
   ProfileEstimator(const PackedDB& rdb, const LasData& rL, uint64_t rmaxalign, uint64_t rmaxinput, uint64_t rvard = 0, uint64_t ravglen = 0)
       : db(rdb), L(rL), maxalign(rmaxalign), maxinput(rmaxinput), vard(rvard), avglen(ravglen), RP(rdb, rL, PileParams()) {}
 
-  // one A-read: adds to C, returns the mean error rate of its consensus windows (0 if none).  recs: if given, one record per window
-  // with a non-empty pile is appended; core: if given, the piles are evaluated by profile_core.cuh (CoreEval) instead of evaluate()
-  double read(uint64_t aread, ProfileCounts& C, std::vector<ProfileWindow>* recs = nullptr, CoreEval* core = nullptr) {
+  // one A-read: appends one record per window with a non-empty pile to recs, in window order (profile_counts sums them); core: if
+  // given, the piles are evaluated by profile_core.cuh (CoreEval) instead of evaluate()
+  void read(uint64_t aread, std::vector<ProfileWindow>& recs, CoreEval* core = nullptr) {
     select_overlaps_profile(L, aread, read_limit(db.rlen[aread], maxinput, vard, avglen), sel);
     const size_t nintv = sel.size();
-    if (!nintv) return 0.0;
+    if (!nintv) return;
     decode_read(db, (uint32_t)aread, false, RP.abuf);
     if (bm.size() < nintv) { bm.resize(nintv); bseq.resize(nintv); }
     uint64_t maxaepos = 0; double maxerate = 0.0, minerate = 1.0;
@@ -313,7 +314,7 @@ class ProfileEstimator {
     }
     const uint64_t ylimit = (maxaepos + EA >= EW) ? (maxaepos + EA - EW) / EA : 0;
     std::map<uint64_t, size_t> active;        // pile order: (scaled error rate, index)
-    size_t z = 0; double esum = 0.0; uint64_t ecnt = 0;
+    size_t z = 0;
     for (uint64_t y = 0; y < ylimit; ++y) {
       const int64_t astart = (int64_t)(y * EA), aend = astart + EW;
       for (; z < nintv && L.ovl[sel[z]].abpos <= astart; ++z)
@@ -331,20 +332,10 @@ class ProfileEstimator {
       }
       uint64_t g[4] = {0, 0, 0, 0};
       const int st = core ? core->run(pile, g) : evaluate(g);
-      if (recs) {
-        ProfileWindow r; r.aread = (uint32_t)aread; r.astart = (uint32_t)astart; r.status = (uint32_t)st; r.reserved = 0;
-        for (int i = 0; i < 4; ++i) r.cnt[i] = (uint32_t)g[i];
-        recs->push_back(r);
-      }
-      if (st == dprof::ST_SKIPPED) continue;
-      if (st == dprof::ST_REPEAT) { C.unusable++; continue; }
-      C.usable++;
-      if (st != dprof::ST_OK) continue;
-      for (int i = 0; i < 4; ++i) C.cnt[i] += g[i];
-      esum += (double)(g[1] + g[2] + g[3]) / (double)(g[0] + g[1] + g[2] + g[3]);
-      ++ecnt;
+      ProfileWindow r; r.aread = (uint32_t)aread; r.astart = (uint32_t)astart; r.status = (uint32_t)st; r.reserved = 0;
+      for (int i = 0; i < 4; ++i) r.cnt[i] = (uint32_t)g[i];
+      recs.push_back(r);
     }
-    return ecnt ? esum / (double)ecnt : 0.0;
   }
 
  private:
@@ -364,37 +355,6 @@ class ProfileEstimator {
   std::vector<Seq> pile; std::vector<uint8_t> cons;
 };
 
-// A-reads [lo, min(hi, lo + 1024)); per-read results are combined in read order whatever the thread count.  vard / avglen: --vard
-// and the DB's average read length (read_limit in pile.hpp; the estimator applies the same per-read limit, src/daccord.cpp:1689-1694)
-inline ProfileCounts estimate_profile(const PackedDB& db, const LasData& L, int64_t lo, int64_t hi, uint64_t maxalign, uint64_t maxinput, int nthreads,
-                                      uint64_t vard = 0, uint64_t avglen = 0) {
-  const int64_t top = std::min(hi, lo + 1024), nr = std::max<int64_t>(top - lo, 0);
-  std::vector<ProfileCounts> per(nr); std::vector<double> rate(nr, 0.0);
-  if (nthreads < 1) nthreads = 1;
-#pragma omp parallel num_threads(nthreads)
-  {
-    ProfileEstimator PE(db, L, maxalign, maxinput, vard, avglen);
-#pragma omp for schedule(dynamic, 1)
-    for (int64_t i = 0; i < nr; ++i) {
-      if (L.aidx[lo + i] == L.aidx[lo + i + 1]) continue;
-      per[i].reads = 1;
-      rate[i] = PE.read((uint64_t)(lo + i), per[i]);
-    }
-  }
-  ProfileCounts R; double s = 0.0; uint64_t n = 0;
-  for (int64_t i = 0; i < nr; ++i) {
-    for (int j = 0; j < 4; ++j) R.cnt[j] += per[i].cnt[j];
-    R.usable += per[i].usable; R.unusable += per[i].unusable; R.reads += per[i].reads;
-    if (rate[i] != 0.0) { s += rate[i]; ++n; }
-  }
-  if (n) {
-    R.eavg = s / (double)n; double d = 0.0;
-    for (int64_t i = 0; i < nr; ++i) if (rate[i] != 0.0) d += (R.eavg - rate[i]) * (R.eavg - rate[i]);
-    R.edif = std::sqrt(d / (double)n);
-  }
-  return R;
-}
-
 // the windows of A-reads [lo, hi) in read order (no cap on the read count); core: evaluate the piles with profile_core.cuh (CoreEval),
 // *host_windows = the windows beyond the GPU kernel's capacities
 inline std::vector<ProfileWindow> profile_windows(const PackedDB& db, const LasData& L, int64_t lo, int64_t hi, uint64_t maxalign, uint64_t maxinput, int nthreads,
@@ -405,17 +365,63 @@ inline std::vector<ProfileWindow> profile_windows(const PackedDB& db, const LasD
 #pragma omp parallel num_threads(nthreads) reduction(+ : hw)
   {
     ProfileEstimator PE(db, L, maxalign, maxinput, vard, avglen);
-    CoreEval CE; ProfileCounts C;
+    CoreEval CE;
 #pragma omp for schedule(dynamic, 1)
     for (int64_t i = 0; i < nr; ++i) {
       if (L.aidx[lo + i] == L.aidx[lo + i + 1]) continue;
-      PE.read((uint64_t)(lo + i), C, &per[i], core ? &CE : nullptr);
+      PE.read((uint64_t)(lo + i), per[i], core ? &CE : nullptr);
     }
     hw += CE.host_windows;
   }
   std::vector<ProfileWindow> R;
   for (auto& v : per) R.insert(R.end(), v.begin(), v.end());
   if (host_windows) *host_windows = hw;
+  return R;
+}
+
+// the error profile of the estimator's window records, in (aread, astart) order -- from the host (profile_windows) or the GPU (dcu_profile)
+// alike (reference src/daccord.cpp:538-630, :1774-1845): usable = windows with a repeat-free pile of >= 3 sequences, unusable = those with a
+// repeated 7-mer, cnt = the step counts of the windows with a consensus.  A read's error rate is the mean of (mis + ins + del) / steps over
+// its consensus windows, summed in window order; eavg / edif are the mean and deviation of the non-zero read rates, summed in read order.
+// `reads` (A-reads with overlaps) is not in the records and stays 0.
+inline ProfileCounts profile_counts(const ProfileWindow* rec, size_t n) {
+  ProfileCounts R;
+  std::vector<double> rate;                   // per read with records
+  for (size_t i = 0; i < n;) {
+    const uint32_t aread = rec[i].aread;
+    double esum = 0.0; uint64_t ecnt = 0;
+    for (; i < n && rec[i].aread == aread; ++i) {
+      const ProfileWindow& r = rec[i];
+      if (r.status == dprof::ST_SKIPPED) continue;
+      if (r.status == dprof::ST_REPEAT) { R.unusable++; continue; }
+      R.usable++;
+      if (r.status != dprof::ST_OK) continue;
+      uint64_t g[4];
+      for (int j = 0; j < 4; ++j) { g[j] = r.cnt[j]; R.cnt[j] += g[j]; }
+      esum += (double)(g[1] + g[2] + g[3]) / (double)(g[0] + g[1] + g[2] + g[3]);
+      ++ecnt;
+    }
+    rate.push_back(ecnt ? esum / (double)ecnt : 0.0);
+  }
+  double s = 0.0; uint64_t m = 0;
+  for (double e : rate) if (e != 0.0) { s += e; ++m; }
+  if (m) {
+    R.eavg = s / (double)m; double d = 0.0;
+    for (double e : rate) if (e != 0.0) d += (R.eavg - e) * (R.eavg - e);
+    R.edif = std::sqrt(d / (double)m);
+  }
+  return R;
+}
+
+// A-reads [lo, min(hi, lo + 1024)) on the host: their window records (profile_windows), summed by profile_counts in read order whatever
+// the thread count.  vard / avglen: --vard and the DB's average read length (read_limit in pile.hpp; the estimator applies the same
+// per-read limit, src/daccord.cpp:1689-1694)
+inline ProfileCounts estimate_profile(const PackedDB& db, const LasData& L, int64_t lo, int64_t hi, uint64_t maxalign, uint64_t maxinput, int nthreads,
+                                      uint64_t vard = 0, uint64_t avglen = 0) {
+  const int64_t top = std::min(hi, lo + 1024);
+  const std::vector<ProfileWindow> rec = profile_windows(db, L, lo, top, maxalign, maxinput, nthreads, vard, avglen, false, nullptr);
+  ProfileCounts R = profile_counts(rec.data(), rec.size());
+  for (int64_t r = lo; r < top; ++r) R.reads += L.aidx[r] != L.aidx[r + 1];
   return R;
 }
 

@@ -287,6 +287,14 @@ ProfileWindow* dh_profile_windows(dh_data* d, int64_t first_read, int64_t last_r
     return out;
   } catch (std::exception& e) { d->err = e.what(); return nullptr; }
 }
+// the error profile of n window records in (aread, astart) order (profile_counts, what daccord sums the GPU's records with):
+// out6 = matches, mismatches, insertions, deletions, usable windows, unusable windows; dout2 = eavg, edif
+void dh_profile_counts(const ProfileWindow* rec, uint64_t n, uint64_t* out6, double* dout2) {
+  const ProfileCounts C = profile_counts(rec, n);
+  for (int i = 0; i < 4; ++i) out6[i] = C.cnt[i];
+  out6[4] = C.usable; out6[5] = C.unusable;
+  dout2[0] = C.eavg; dout2[1] = C.edif;
+}
 int dh_estimate_profile(dh_data* d, int64_t first_read, int64_t last_read, uint64_t maxalign, uint64_t maxinput, int nthreads, uint64_t* out7, double* dout2) {
   return dh_estimate_profile_vard(d, first_read, last_read, maxalign, maxinput, 0, nthreads, out7, dout2);
 }

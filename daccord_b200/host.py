@@ -218,6 +218,20 @@ def read_eprof(path):
     return [int(x) for x in a]
 
 
+def profile_counts(records):
+    """the error profile of the estimator's window records (daccord_b200.PROFILE_WINDOW_DT in (aread, astart) order, e.g. from
+    Dataset.profile_windows or Engine.profile), summed the way daccord sums them: the keys of Dataset.estimate_profile except 'reads'"""
+    from . import PROFILE_WINDOW_DT
+    rec = np.ascontiguousarray(records, dtype=PROFILE_WINDOW_DT)
+    a = (C.c_uint64 * 6)()
+    d = (C.c_double * 2)()
+    lib().dh_profile_counts(rec.ctypes.data_as(C.c_void_p), C.c_uint64(len(rec)), a, d)
+    keys = ("matches", "mismatches", "insertions", "deletions", "usable", "unusable")
+    out = {k: int(v) for k, v in zip(keys, a)}
+    out["eavg"], out["edif"] = float(d[0]), float(d[1])
+    return out
+
+
 def format_segments(seg, chars, counter=0):
     """FastA text (bytes) of the segments returned by Engine.vote; returns (fasta, next counter)"""
     c = C.c_uint64(counter)

@@ -75,6 +75,9 @@ typedef struct dcu_ctx dcu_ctx;
  * src/daccord.cpp:1867-1913, :1981-1988 + per-thread HandleContext construction :1989-2023) */
 int dcu_create(const dcu_params* params, int device, dcu_ctx** out);
 void dcu_destroy(dcu_ctx* ctx);
+/* number of CUDA devices this process sees.  *n = 0 and DCU_OK when the runtime reports no device (e.g. CUDA_VISIBLE_DEVICES="")
+ * or no driver, so a caller can pick a host path; any other CUDA error is DCU_ERR_CUDA.  Creates no context. */
+int dcu_device_count(int* n);
 /* packed 2-bit read database, Dazzler .bps layout: 4 bases per byte, first base in the top
  * two bits (replaces DecodedReadContainer, reference src/DecodedReadContainer.hpp:81-84).
  * Two databases (an asymmetric .las, `daligner A.db B.db`): pass A's bytes followed by B's; to dcu_pile / dcu_vote pass the
