@@ -60,35 +60,59 @@ struct KArgs {
   unsigned int launch_seq;             // number of this launch in the context's life (upper half of the forward slot tags: records of earlier launches in the slab are stale)
 };
 
+// Per-stage clocks of the window kernels (-DDCU_STAGE_CLOCKS, a measurement build next to the product library, read by
+// tools/stage_clocks.py): clock64() around every stage call and every group barrier, summed per warp in shared memory and added to
+// g_stage_clk when the warp leaves the kernel.  clock64() is per SM: only differences taken by one warp are summed.  Without the
+// switch the macros expand to the bare statement and the kernels are the product's, instruction for instruction.
+// Slots: busy cycles of the nine stages, their calls, wait cycles at the round barrier (slot CLK_WAIT) and at the barrier behind each of
+// the first eight stages, fetch (ticket, st_begin, publish), barrier waits of a warp that has no window left, the warp's whole life.
+#ifdef DCU_STAGE_CLOCKS
+enum { CLK_BUSY = 0, CLK_CALLS = 9, CLK_WAIT = 18, CLK_FETCH = 27, CLK_IDLE = 28, CLK_LIFE = 29, CLK_N = 30 };
+__device__ unsigned long long g_stage_clk[CLK_N];
+#define DCU_CLK_DECL(NW) __shared__ unsigned long long s_clk[NW][CLK_N]; if (lane == 0) for (int i_ = 0; i_ < CLK_N; ++i_) s_clk[warp][i_] = 0; const long long clk_life_ = clock64();
+#define DCU_CLK_STAGE(i, call) do { const long long t0_ = clock64(); call; if (lane == 0) { s_clk[warp][CLK_BUSY + (i)] += (unsigned long long)(clock64() - t0_); s_clk[warp][CLK_CALLS + (i)] += 1; } } while (0)
+#define DCU_CLK_WAIT(i, call) do { const long long t0_ = clock64(); call; if (lane == 0) s_clk[warp][idle ? (int)CLK_IDLE : CLK_WAIT + (i)] += (unsigned long long)(clock64() - t0_); } while (0)
+#define DCU_CLK_FETCH_BEGIN const long long clk_f0_ = clock64();
+#define DCU_CLK_FETCH_END if (lane == 0) s_clk[warp][CLK_FETCH] += (unsigned long long)(clock64() - clk_f0_);
+#define DCU_CLK_FLUSH if (lane == 0) { s_clk[warp][CLK_LIFE] = (unsigned long long)(clock64() - clk_life_); for (int i_ = 0; i_ < CLK_N; ++i_) atomicAdd(&g_stage_clk[i_], s_clk[warp][i_]); }
+#else
+#define DCU_CLK_DECL(NW)
+#define DCU_CLK_STAGE(i, call) call
+#define DCU_CLK_WAIT(i, call) call
+#define DCU_CLK_FETCH_BEGIN
+#define DCU_CLK_FETCH_END
+#define DCU_CLK_FLUSH
+#endif
+
 // One persistent launch per pass.  Every warp owns one window at a time and walks it through the stages of window_core.cuh; the
 // warps of a group (named barriers) run the same stage at the same time, which keeps the instruction caches effective
 // (the kernel is ~190 KB of SASS, a stage a few KB of it).  NS = dcu (HBM workspace) or dcus (hot fields in shared memory, slices staged by bulk copies).
-#define DCU_STAGE_LOOP(NS, FINAL_HOOK)                                                                                          \
-    if (G == 1) alldone = idle;                                                                                                 \
-    else {                                                                                                                      \
-      if (lane == 0) s_done[par][warp] = idle ? 1 : 0;                                                                          \
-      gsync();                                                                                                                  \
-      alldone = true;                                                                                                           \
-      for (int i = 0; i < G; ++i) alldone = alldone && (s_done[par][gfirst + i] != 0);                                          \
-    }                                                                                                                           \
-    if (alldone) break;                                                                                                         \
-    if (st.ph == NS::PH_HASH) NS::st_hash(c, st, lane);                                                                         \
-    if (smask & 1) gsync();                                                                                                     \
-    if (st.ph == NS::PH_NODES) NS::st_nodes(c, st, lane);                                                                       \
-    if (smask & 32) gsync();                                                                                                    \
-    if (st.ph == NS::PH_EDGES) NS::st_edges(c, st, lane);                                                                       \
-    if (smask & 2) gsync();                                                                                                     \
-    if (st.ph == NS::PH_TRAV) NS::st_trav(c, st, lane);                                                                         \
-    if (smask & 16) gsync();                                                                                                    \
-    if (st.ph == NS::PH_POS) NS::st_pos(c, st, lane);                                                                           \
-    if (smask & 4) gsync();                                                                                                     \
-    if (st.ph == NS::PH_RPATH) NS::st_rpath(c, st, lane);                                                                       \
-    if (smask & 64) gsync();                                                                                                    \
-    if (st.ph == NS::PH_SEARCH) NS::st_search(c, st, lane);                                                                     \
-    if (smask & 128) gsync();                                                                                                   \
-    if (st.ph == NS::PH_SCORE) NS::st_score(c, st, lane);                                                                       \
-    if (smask & 8) gsync();                                                                                                     \
-    if (st.ph == NS::PH_FINAL) { FINAL_HOOK; NS::st_final(c, st, a.cons + (size_t)wi * DCU_CONS_STRIDE, a.ops + (size_t)wi * DCU_OPS_STRIDE, lane); } \
+#define DCU_STAGE_LOOP(NS, FINAL_HOOK)                                                                                                                                  \
+    if (G == 1) alldone = idle;                                                                                                                                         \
+    else {                                                                                                                                                              \
+      if (lane == 0) s_done[par][warp] = idle ? 1 : 0;                                                                                                                  \
+      DCU_CLK_WAIT(0, gsync());                                                                                                                                         \
+      alldone = true;                                                                                                                                                   \
+      for (int i = 0; i < G; ++i) alldone = alldone && (s_done[par][gfirst + i] != 0);                                                                                  \
+    }                                                                                                                                                                   \
+    if (alldone) break;                                                                                                                                                 \
+    if (st.ph == NS::PH_HASH) DCU_CLK_STAGE(0, NS::st_hash(c, st, lane));                                                                                               \
+    if (smask & 1) DCU_CLK_WAIT(1, gsync());                                                                                                                            \
+    if (st.ph == NS::PH_NODES) DCU_CLK_STAGE(1, NS::st_nodes(c, st, lane));                                                                                             \
+    if (smask & 32) DCU_CLK_WAIT(2, gsync());                                                                                                                           \
+    if (st.ph == NS::PH_EDGES) DCU_CLK_STAGE(2, NS::st_edges(c, st, lane));                                                                                             \
+    if (smask & 2) DCU_CLK_WAIT(3, gsync());                                                                                                                            \
+    if (st.ph == NS::PH_TRAV) DCU_CLK_STAGE(3, NS::st_trav(c, st, lane));                                                                                               \
+    if (smask & 16) DCU_CLK_WAIT(4, gsync());                                                                                                                           \
+    if (st.ph == NS::PH_POS) DCU_CLK_STAGE(4, NS::st_pos(c, st, lane));                                                                                                 \
+    if (smask & 4) DCU_CLK_WAIT(5, gsync());                                                                                                                            \
+    if (st.ph == NS::PH_RPATH) DCU_CLK_STAGE(5, NS::st_rpath(c, st, lane));                                                                                             \
+    if (smask & 64) DCU_CLK_WAIT(6, gsync());                                                                                                                           \
+    if (st.ph == NS::PH_SEARCH) DCU_CLK_STAGE(6, NS::st_search(c, st, lane));                                                                                           \
+    if (smask & 128) DCU_CLK_WAIT(7, gsync());                                                                                                                          \
+    if (st.ph == NS::PH_SCORE) DCU_CLK_STAGE(7, NS::st_score(c, st, lane));                                                                                             \
+    if (smask & 8) DCU_CLK_WAIT(8, gsync());                                                                                                                            \
+    if (st.ph == NS::PH_FINAL) { FINAL_HOOK; DCU_CLK_STAGE(8, NS::st_final(c, st, a.cons + (size_t)wi * DCU_CONS_STRIDE, a.ops + (size_t)wi * DCU_OPS_STRIDE, lane)); } \
     if (st.ph == NS::PH_END && !idle) { publish(); __syncwarp(); }
 
 // ---- HBM build: layout, capacities, table descriptors and parameters in __constant__ memory (dcu::c_*), set per launch
@@ -106,6 +130,7 @@ template <int W, int B = BPS> __global__ void __launch_bounds__(W * 32, B) dcu_w
   auto gsync = [&]() { if (G > 1) asm volatile("bar.sync %0, %1;" ::"r"(grp + 1), "r"(G * 32) : "memory"); };
   const int smask = a.sync_mask;                       // which of the inner stage boundaries are barriers (bit 0: hash|nodes, 5: nodes|edges, 1: edges|trav, 4: trav|pos, 2: pos|rpath, 6: rpath|search, 7: search|score, 3: score|final)
   dcu::WinState st; st.ph = dcu::PH_END;
+  DCU_CLK_DECL(W)
   uint32_t wi = 0; bool nomore = false; int par = 0;
   auto publish = [&]() {
     if (lane == 0) {
@@ -114,6 +139,7 @@ template <int W, int B = BPS> __global__ void __launch_bounds__(W * 32, B) dcu_w
     }
   };
   for (;; par ^= 1) {
+    DCU_CLK_FETCH_BEGIN
     while (!nomore && st.ph == dcu::PH_END) {          // finish / fetch
       unsigned int t = 0;
       if (lane == 0) t = atomicAdd(a.ticket, 1u);
@@ -124,10 +150,12 @@ template <int W, int B = BPS> __global__ void __launch_bounds__(W * 32, B) dcu_w
       dcu::st_begin(c, st, wd, lane, nullptr);
       if (st.ph == dcu::PH_END) publish();             // skipped or overflowed right away
     }
+    DCU_CLK_FETCH_END
     const bool idle = st.ph == dcu::PH_END;
     bool alldone;
     DCU_STAGE_LOOP(dcu, (void)0)
   }
+  DCU_CLK_FLUSH
 }
 
 // ---- hybrid build: as dcu_window_kernel, plus a 5 KB arena per warp behind the VS table that holds the window's k-mer table
@@ -145,6 +173,7 @@ __global__ void __launch_bounds__(WPB * 32, BPS) dcuh_window_kernel(const __grid
   auto gsync = [&]() { if (G > 1) asm volatile("bar.sync %0, %1;" ::"r"(grp + 1), "r"(G * 32) : "memory"); };
   const int smask = a.sync_mask;
   dcuh::WinState st; st.ph = dcuh::PH_END;
+  DCU_CLK_DECL(WPB)
   uint32_t wi = 0; bool nomore = false; int par = 0;
   auto publish = [&]() {
     if (lane == 0) {
@@ -153,6 +182,7 @@ __global__ void __launch_bounds__(WPB * 32, BPS) dcuh_window_kernel(const __grid
     }
   };
   for (;; par ^= 1) {
+    DCU_CLK_FETCH_BEGIN
     while (!nomore && st.ph == dcuh::PH_END) {         // finish / fetch
       unsigned int t = 0;
       if (lane == 0) t = atomicAdd(a.ticket, 1u);
@@ -163,10 +193,12 @@ __global__ void __launch_bounds__(WPB * 32, BPS) dcuh_window_kernel(const __grid
       dcuh::st_begin(c, st, wd, lane, nullptr);
       if (st.ph == dcuh::PH_END) publish();
     }
+    DCU_CLK_FETCH_END
     const bool idle = st.ph == dcuh::PH_END;
     bool alldone;
     DCU_STAGE_LOOP(dcuh, (void)0)
   }
+  DCU_CLK_FLUSH
 }
 
 // ---- wide build: as dcu_window_kernel with 32-bit slice offsets and counts, always free running (the windows are few and uneven)
@@ -183,6 +215,7 @@ __global__ void __launch_bounds__(WWPB * 32) dcuw_window_kernel(const __grid_con
   auto gsync = [&]() {};
   const int smask = 0;
   dcuw::WinState st; st.ph = dcuw::PH_END;
+  DCU_CLK_DECL(WWPB)
   uint32_t wi = 0; bool nomore = false; int par = 0;
   auto publish = [&]() {
     if (lane == 0) {
@@ -191,6 +224,7 @@ __global__ void __launch_bounds__(WWPB * 32) dcuw_window_kernel(const __grid_con
     }
   };
   for (;; par ^= 1) {
+    DCU_CLK_FETCH_BEGIN
     while (!nomore && st.ph == dcuw::PH_END) {
       unsigned int t = 0;
       if (lane == 0) t = atomicAdd(a.ticket, 1u);
@@ -201,10 +235,12 @@ __global__ void __launch_bounds__(WWPB * 32) dcuw_window_kernel(const __grid_con
       dcuw::st_begin(c, st, wd, lane, nullptr);
       if (st.ph == dcuw::PH_END) publish();
     }
+    DCU_CLK_FETCH_END
     const bool idle = st.ph == dcuw::PH_END;
     bool alldone;
     DCU_STAGE_LOOP(dcuw, (void)0)
   }
+  DCU_CLK_FLUSH
 }
 
 // ---- shared-memory build: dynamic shared memory = [transposed VS table | one arena per warp]; the packed bytes of the next
@@ -234,6 +270,7 @@ __global__ void __launch_bounds__(SWPB * 32, 1) dcus_window_kernel(const __grid_
   auto gsync = [&]() { if (G > 1) asm volatile("bar.sync %0, %1;" ::"r"(grp + 1), "r"(G * 32) : "memory"); };
   const int smask = a.sync_mask;
   dcus::WinState st; st.ph = dcus::PH_END;
+  DCU_CLK_DECL(SWPB)
   uint32_t wi = 0; bool nomore = false; int par = 0;
   // staging state: pf = 0 nothing claimed, 1 window pfwi claimed and its slices in flight / landed, 2 claimed but not staged (direct loads)
   int pf = 0; uint32_t pfwi = 0, mpar = 0;
@@ -282,6 +319,7 @@ __global__ void __launch_bounds__(SWPB * 32, 1) dcus_window_kernel(const __grid_
     pf = 1;
   };
   for (;; par ^= 1) {
+    DCU_CLK_FETCH_BEGIN
     while (st.ph == dcus::PH_END) {                    // finish / fetch
       if (pf == 0) { if (nomore) break; claim(); if (pf == 0) break; }
       const uint8_t* rawp = nullptr;
@@ -294,10 +332,12 @@ __global__ void __launch_bounds__(SWPB * 32, 1) dcus_window_kernel(const __grid_
       dcus::st_begin(c, st, W, lane, rawp);
       if (st.ph == dcus::PH_END) publish();            // skipped or overflowed right away
     }
+    DCU_CLK_FETCH_END
     const bool idle = st.ph == dcus::PH_END;
     bool alldone;
     DCU_STAGE_LOOP(dcus, if (pf == 0 && !nomore) claim())
   }
+  DCU_CLK_FLUSH
 }
 
 // ---------------------------------------------------------------- piling kernels (pile_core.cuh), one thread per item
@@ -1284,5 +1324,17 @@ int64_t dcu_get_tables(dcu_ctx* ctx, int which, double* out, int64_t cap) {
   if (!ok) { ctx->err = "dcu_get_tables: device to host copy failed"; return -1; }
   return (int64_t)n;
 }
+
+#ifdef DCU_STAGE_CLOCKS
+// measurement build only: copies the CLK_N counters of the window kernels (summed over all launches since the last reset) to out, then zeroes them
+int dcu_stage_clocks(dcu_ctx* ctx, uint64_t* out, int n, int reset) {
+  if (!ctx || !out || n != CLK_N) return DCU_ERR_PARAM;
+  CK(cudaSetDevice(ctx->device));
+  CK(cudaStreamSynchronize(ctx->stream));
+  CK(cudaMemcpyFromSymbol(out, g_stage_clk, sizeof(unsigned long long) * CLK_N));
+  if (reset) { const unsigned long long z[CLK_N] = {}; CK(cudaMemcpyToSymbol(g_stage_clk, z, sizeof(z))); }
+  return DCU_OK;
+}
+#endif
 
 }  // extern "C"

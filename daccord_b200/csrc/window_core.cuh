@@ -1130,31 +1130,55 @@ DCU_NOINL void sp_view(const Ctx& c, int off, int L, int nr, int br, uint32_t cO
 #endif
   sp_view_t<false>(c, off, L, nr, br, cO, lane);
 }
-// one forward slot: stretch s anchored at true position p (one lane; the forward search calls this the first time it looks at a slot)
-template <bool SM> DCU_FN FSlot fwd_slot_eval_t(const Ctx& c, int s, int p, unsigned long long tag) {
+// one forward slot: stretch s anchored at true position p (the forward search calls this the first time it looks at a slot).  Warp-uniform
+// arguments, every lane returns the record.  The links are taken 32 at a time; when fewer are left, G lanes share a link (unitigs are short:
+// a median of three links, each with as many instances as the pile is deep).  The G lanes split the link's instance list and add their
+// parts -- a sum of 64-bit integers, exact in any order.  A ballot finds the first link that fails, and the weights before it are added in
+// link order, each taken from its lanes by a shuffle: the additions a single lane walking the links would make.  Links behind a failing
+// one are weighed in vain; they touch nothing.
+template <bool SM> DCU_FN FSlot fwd_slot_eval_t(const Ctx& c, int s, int p, unsigned long long tag, int lane) {
   const WS w = c.ws;
   const int NP = DCU_T.NP, MS = DCU_T.MS;
   const int off = w.ds_off()[s], L = w.ds_len()[s];
+  const uint32_t row = (uint32_t)NP * 8u;
   FSlot r; r.w = -1.0; r.wf = 0.0; r.wl = 0.0; r.epoch = tag;
   double sum = 0.0;
   DCU_NOUNROLL
-  for (int jj = 0; jj < L; ++jj) {                     // link jj at true position p + jj
-    const int n = w.slinks()[off + jj], pp = p + jj;
-    double wt = 0.0;
-    if (pp < NP) wt = (double)inst_colsum<SM>(c, w.ipos() + w.n_ioff()[n], (int)w.n_freq()[n], pp, NP, MS) * 2.3283064365386963e-10;
-    if (!(wt >= 1e-3)) return r;
-    sum += wt;
-    if (jj == 0) r.wf = wt;
-    if (jj == L - 1) r.wl = wt;
+  for (int j0 = 0; j0 < L; j0 += DCU_NL) {
+    const int jn = L - j0 < DCU_NL ? L - j0 : DCU_NL;
+    int G = 1; while (2 * G * jn <= DCU_NL) G *= 2;
+    const int jj = j0 + lane / G, sub = lane % G, pp = p + jj;      // link jj at true position p + jj
+    const bool live = jj < L && pp < NP;
+    unsigned long long u = 0;
+    if (live) {
+      const int n = w.slinks()[off + jj], f = (int)w.n_freq()[n];
+      const uint8_t* ip = w.ipos() + w.n_ioff()[n];
+      const uint8_t* col = vs_col<SM>(c, pp);
+      DCU_NOUNROLL
+      for (int t = sub; t < f; t += G) { int a = ip[t]; a = a < MS ? a : MS; u += *(const unsigned long long*)(col + (uint32_t)a * row); }
+    }
+    DCU_NOUNROLL
+    for (int o = G >> 1; o > 0; o >>= 1) u += bcast(u, lane ^ o);
+    const double wt = live ? (double)u * 2.3283064365386963e-10 : 0.0;
+    const uint32_t fail = ballot(sub == 0 && jj < L && !(wt >= 1e-3));
+    const int nok = fail ? popc((fail - 1u) & ~fail) / G : jn;      // links of this group before the first failing one
+    DCU_NOUNROLL
+    for (int t = 0; t < nok; ++t) {
+      const double x = bcast(wt, t * G);
+      sum += x;
+      if (j0 + t == 0) r.wf = x;
+      if (j0 + t == L - 1) r.wl = x;
+    }
+    if (fail) return r;
   }
   r.w = sum;
   return r;
 }
-DCU_NOINL FSlot fwd_slot_eval(const Ctx& c, int s, int p, unsigned long long tag) {
+DCU_NOINL FSlot fwd_slot_eval(const Ctx& c, int s, int p, unsigned long long tag, int lane) {
 #ifndef DCU_EMU
-  if (c.vs_sm) return fwd_slot_eval_t<true>(c, s, p, tag);
+  if (c.vs_sm) return fwd_slot_eval_t<true>(c, s, p, tag, lane);
 #endif
-  return fwd_slot_eval_t<false>(c, s, p, tag);
+  return fwd_slot_eval_t<false>(c, s, p, tag, lane);
 }
 // The slots of a view depend on its links only, not on the (first,last) pair, and a pair splits at most the two unitigs that hold
 // its first / last k-mer as an interior node: the slots of the raw unitigs are therefore computed once per traverse (the first
@@ -1236,14 +1260,16 @@ DCU_BIG void stretch_positions(Ctx& c, int lane) {
   }
   wsync();
 }
-DCU_NOINL int sfo_fwd(const Ctx& c, int s, int p) {     // getCachedStretchPositionWeight (:3906-3918); evaluates the slot at its first use
+// getCachedStretchPositionWeight (:3906-3918); evaluates the slot at its first use.  Warp-uniform: all lanes look at the record, the warp
+// evaluates a missing one together (the collectives of the evaluation lie between the lanes' look at the old record and the store of the new)
+DCU_NOINL int sfo_fwd(const Ctx& c, int s, int p, int lane) {
   const WS w = c.ws; int d = p - (int)w.ds_fB()[s];
   if (d < 0 || d >= (int)w.ds_fN()[s]) return -1;
   const uint32_t o = w.ds_fO()[s] + (uint32_t)d;
   const unsigned long long tag = o < c.fbase0 ? c.epoch_trav : c.epoch_pair;
   double wt;
   if (w.sfs()[o].epoch == tag) wt = w.sfs()[o].w;
-  else { const FSlot r = fwd_slot_eval(c, s, p, tag); w.sfs()[o] = r; wt = r.w; }
+  else { const FSlot r = fwd_slot_eval(c, s, p, tag, lane); if (lane == 0) w.sfs()[o] = r; wsync(); wt = r.w; }
   return wt >= 0.0 ? (int)o : -1;
 }
 DCU_NOINL int sfo_rev(const Ctx& c, int s, int p) {     // getCachedStretchReversePositionWeight (:3920-3932)
@@ -1363,69 +1389,93 @@ DCU_FN Peq make_peq_packed(const uint32_t* t, int m) {      // a slice of the wi
 // ------------------------------------------------------------------ traverse (:4496-5170)
 struct TravOut { int nacc; };
 
-DCU_NOINL int rp_new(Ctx& c, int& nrp, double wgt, uint32_t parent, uint32_t front, int stretch, int pos, int len, int baselen) {
-  const WS w = c.ws;
-  DCU_PEAK(8, nrp + 1);
-  if (nrp >= DCU_CAP.RP) { c.overflow = 11; return -1; }
-  int id = nrp++;
+DCU_FN void rp_store(const WS& w, int id, double wgt, uint32_t parent, uint32_t front, int stretch, int pos, int len, int baselen) {
   w.rp_w()[id] = wgt; w.rp_parent()[id] = parent; w.rp_front()[id] = front; w.rp_stretch()[id] = (uint16_t)stretch;
   w.rp_pos()[id] = (uint16_t)pos; w.rp_len()[id] = (uint16_t)len; w.rp_baselen()[id] = (uint16_t)baselen;
-  return id;
+}
+// heap_push / heap_pop by lane 0 for a warp whose lanes all hold n: the wsync() before keeps the other lanes' earlier reads of the heap
+// ahead of the stores, the one after the stores ahead of everybody's later reads.  (tools/lane_mutants.py: the test data never shows the
+// loss of the one before a push -- today every caller has passed a sync since it last read that heap -- nor of the one after a pop,
+// which only matters where the next read of the heap top follows without a collective: an inert path in reverse_paths, a candidate
+// below a full candidate heap in search_pair.)
+DCU_FN void heap_push_l0(bool MAXH, double* hw, uint32_t* hi, int& n, double w, uint32_t id, int lane) {
+  wsync();
+  if (lane == 0) heap_push(MAXH, hw, hi, n, w, id); else ++n;
+  wsync();
+}
+DCU_FN void heap_pop_l0(bool MAXH, double* hw, uint32_t* hi, int& n, int lane) {
+  wsync();
+  if (lane == 0) heap_pop(MAXH, hw, hi, n); else --n;
+  wsync();
 }
 
-// reverse half-paths (prepareTraverse :3576-3757); lane 0
-DCU_BIG void reverse_paths(Ctx& c, int Lnode, int lmax, int& narp, int nseed) {
+// The two searches (reverse_paths, search_pair) run on all lanes: every lane walks the same control flow on the same values (loads of
+// the search state are warp-uniform addresses), lane 0 stores the state, and a wsync() or a collective stands between a store and any
+// other lane's access to the same data, before or after.  What has an order -- the heaps, the ids of the path records, every sum of
+// doubles -- keeps it; the loops that have none (scans, range counts, slot look-ups and weights, string copies) are split over the lanes.
+
+// reverse half-paths (prepareTraverse :3576-3757).  The stretches that may extend a path are looked at by one lane each; the accepted
+// ones get their records and their places in the queue in list order, as if one lane had walked the list.
+DCU_BIG void reverse_paths(Ctx& c, int Lnode, int lmax, int& narp, int nseed, int lane) {
   const WS w = c.ws;
   int nrp = 0, nq = 0; narp = 0;
   DCU_NOUNROLL
-  for (int i = 0; i < DCU_CAP.BL; ++i) w.arph_n()[i] = 0;
-  int seed = rp_new(c, nrp, 0.0, IDX_NONE, w.n_kmer()[Lnode], NID_NONE, 0, 0, c.k);
-  if (seed < 0) return;
-  heap_push(true, w.rq_w(), w.rq_id(), nq, 0.0, (uint32_t)seed);
+  for (int i = lane; i < DCU_CAP.BL; i += DCU_NL) w.arph_n()[i] = 0;
+  DCU_PEAK(8, 1);
+  if (DCU_CAP.RP < 1) { c.overflow = 11; return; }
+  if (lane == 0) rp_store(w, 0, 0.0, IDX_NONE, w.n_kmer()[Lnode], NID_NONE, 0, 0, c.k);
+  nrp = 1;
+  heap_push_l0(true, w.rq_w(), w.rq_id(), nq, 0.0, 0u, lane);
   DCU_NOUNROLL
   while (nq > 0 && !c.overflow) {
     double wt = w.rq_w()[0]; int id = (int)w.rq_id()[0];
-    heap_pop(true, w.rq_w(), w.rq_id(), nq);
+    heap_pop_l0(true, w.rq_w(), w.rq_id(), nq, lane);
     int bl = w.rp_baselen()[id];
     if (bl >= DCU_CAP.BL) continue;                       // longer than any admissible pairing, inert
     double* hw = w.arph_w() + bl * HEAPK; int hn = w.arph_n()[bl];
     if (hn == HEAPK) {                                  // bounded per-length heap (:3626-3665); only weights matter
-      int mi = 0;
+      double mv = 0; int mi = HEAPK;                    // its smallest weight, the first of equals: lanes over the entries
       DCU_NOUNROLL
-      for (int t = 1; t < HEAPK; ++t) if (hw[t] < hw[mi]) mi = t;
-      if (wt <= hw[mi]) continue;
-      hw[mi] = wt;
-    } else { hw[hn] = wt; w.arph_n()[bl] = (uint8_t)(hn + 1); }
-    w.arp()[narp++] = (uint32_t)id;
-    int rlen = w.rp_len()[id], rpos = w.rp_pos()[id];
-    if (rlen == 0) {
-      DCU_NOUNROLL
-      for (int qs = 0; qs < nseed; ++qs) {              // stretches that end in Lnode, ascending (listed by trav_pair_rpaths)
-        const int s = w.dt_len()[qs];
-        int o = sfo_rev(c, s, rpos);                    // extendReversePath (:4058-4105) + feasibility (:4130-4159)
-        if (o >= 0 && w.scs()[o].w >= 0.5) {
-          int L = w.ds_len()[s];
-          int nid = rp_new(c, nrp, w.scs()[o].w, (uint32_t)id, w.n_kmer()[ds_first(c, s)], s, rpos + L - 1, 1, L + c.k - 1);
-          if (nid < 0) return;
-          if (nq >= DCU_CAP.RP) { c.overflow = 12; return; }
-          heap_push(true, w.rq_w(), w.rq_id(), nq, w.scs()[o].w, (uint32_t)nid);
-        }
+      for (int t = lane; t < HEAPK; t += DCU_NL) { const double x = hw[t]; if (mi == HEAPK || x < mv) { mv = x; mi = t; } }
+      double rv = mi < HEAPK ? -mv : -DBL_MAX;
+      red_argmax_d(rv, mi);
+      if (wt <= -rv) continue;
+      if (lane == 0) hw[mi] = wt;
+    } else {
+      wsync();                                          // every lane has read the count
+      if (lane == 0) { hw[hn] = wt; w.arph_n()[bl] = (uint8_t)(hn + 1); }
+    }
+    if (lane == 0) w.arp()[narp] = (uint32_t)id;
+    ++narp;
+    const int rlen = w.rp_len()[id], rpos = w.rp_pos()[id];
+    const bool first = rlen == 0;                       // first step: the stretches that end in Lnode, ascending (listed by trav_pair_rpaths); later: the links into the path's front stretch
+    if (!first && !(bl < (lmax + 1) / 2)) continue;
+    const int ls = first ? 0 : (int)w.rp_stretch()[id];
+    const int t0 = first ? 0 : (int)w.ds_rlO()[ls], tn = first ? nseed : (int)w.ds_rlN()[ls];
+    DCU_NOUNROLL
+    for (int base = 0; base < tn; base += DCU_NL) {
+      const int t = base + lane;
+      bool acc = false; int s = 0; double nw = 0.0;
+      if (t < tn) {
+        s = first ? (int)w.dt_len()[t] : (int)(w.rl()[t0 + t] & 0xFFFF);
+        const int o = sfo_rev(c, s, rpos);              // extendReversePath (:4058-4105) + feasibility (:4130-4159)
+        if (o >= 0 && w.scs()[o].w >= 0.5) { acc = true; nw = first ? w.scs()[o].w : wt + (w.scs()[o].w - w.scs()[o].wf); }
       }
-    } else if (bl < (lmax + 1) / 2) {
-      int ls = w.rp_stretch()[id];
-      DCU_NOUNROLL
-      for (int t = w.ds_rlO()[ls], te = w.ds_rlO()[ls] + w.ds_rlN()[ls]; t < te; ++t) {
-        int s = (int)(w.rl()[t] & 0xFFFF);
-        int o = sfo_rev(c, s, rpos);
-        if (o >= 0 && w.scs()[o].w >= 0.5) {
-          int L = w.ds_len()[s];
-          double nw = wt + (w.scs()[o].w - w.scs()[o].wf);
-          int nid = rp_new(c, nrp, nw, (uint32_t)id, w.n_kmer()[ds_first(c, s)], s, rpos + L - 1, rlen + 1, bl + L - 1);
-          if (nid < 0) return;
-          if (nq >= DCU_CAP.RP) { c.overflow = 13; return; }
-          heap_push(true, w.rq_w(), w.rq_id(), nq, nw, (uint32_t)nid);
-        }
+      const uint32_t ab = ballot(acc);
+      const int cnt = popc(ab);
+      if (!cnt) continue;
+      DCU_PEAK(8, nrp + cnt);
+      if (nrp + cnt > DCU_CAP.RP) { c.overflow = 11; return; }
+      if (nq + cnt > DCU_CAP.RP) { c.overflow = first ? 12 : 13; return; }
+      if (acc) {
+        const int L = w.ds_len()[s];
+        rp_store(w, nrp + popc(ab & lanemask_lt(lane)), nw, (uint32_t)id, w.n_kmer()[ds_first(c, s)], s, rpos + L - 1, first ? 1 : rlen + 1, first ? L + c.k - 1 : bl + L - 1);
       }
+      wsync();
+      if (lane == 0) { DCU_NOUNROLL for (int j = 0; j < cnt; ++j) heap_push(true, w.rq_w(), w.rq_id(), nq, w.rp_w()[nrp + j], (uint32_t)(nrp + j)); }
+      else nq += cnt;
+      nrp += cnt;
+      wsync();
     }
   }
 }
@@ -1454,29 +1504,32 @@ DCU_BIG void sort_reverse_paths(Ctx& c, int narp, int lane) {
   wsync();
 }
 
-DCU_NOINL double pair_score(const Ctx& c, int P, int rpid) {      // getPairScore (:3482-3497)
+DCU_NOINL double pair_score(const Ctx& c, int P, int rpid, int lane) {      // getPairScore (:3482-3497)
   const WS w = c.ws;
   int ls = w.fp_stretch()[P];
   int lpos = w.fp_pos()[P] - (w.ds_len()[ls] - 1);
-  int o = sfo_fwd(c, ls, lpos);
+  int o = sfo_fwd(c, ls, lpos, lane);
   double s = w.fp_w()[P] + w.rp_w()[rpid];
   return o >= 0 ? (s - w.sfs()[o].wl) : s;
 }
-// best / next-best reverse path of an interval in (weight, sorted index) order (:3499-3534)
-DCU_NOINL int interval_next(const Ctx& c, int left, int right, int cur) {
+// best / next-best reverse path of an interval in (weight, sorted index) order (:3499-3534): lanes over the interval, then the largest
+// of the lanes' bests under the same order (a total order: larger weight, then larger index)
+DCU_NOINL int interval_next(const Ctx& c, int left, int right, int cur, int lane) {
   const WS w = c.ws;
   int best = -1; double bw = 0;
   const double* wt = w.arp_wt();
   double cw = cur >= 0 ? wt[cur] : 0;
   DCU_NOUNROLL
-  for (int i = left; i < right; ++i) {
+  for (int i = left + lane; i < right; i += DCU_NL) {
     double wi = wt[i];
     if (cur >= 0 && !(wi < cw || (wi == cw && i < cur))) continue;
     if (best < 0 || wi > bw || (wi == bw && i > best)) { best = i; bw = wi; }
   }
-  return best;
+  double rv = best < 0 ? -DBL_MAX : bw; int ri = best < 0 ? 1 : -best;      // red_argmax_d prefers the smaller index among equal weights: hand it -index
+  red_argmax_d(rv, ri);
+  return ri > 0 ? -1 : -ri;
 }
-DCU_NOINL void apq_push(Ctx& c, int pid) {                        // :4843-4862, :4997-5017
+DCU_NOINL void apq_push(Ctx& c, int pid) {                        // :4843-4862, :4997-5017; one lane
   const WS w = c.ws;
   int bl = w.fp_baselen()[pid];
   if (bl >= DCU_CAP.BL) return;                                  // longer than lmax: never pairs, never extends
@@ -1486,10 +1539,15 @@ DCU_NOINL void apq_push(Ctx& c, int pid) {                        // :4843-4862,
   else heap_push(false, hw, hi, n, wt, (uint32_t)pid);
   w.apq_n()[bl] = (uint8_t)n;
 }
-DCU_NOINL int fp_extend(Ctx& c, int& nfp, int P, int s) {         // extendPath (:3989-4056); P == -1 -> empty path
+DCU_FN void apq_push_l0(Ctx& c, int pid, int lane) {              // (the first wsync also puts the record fp_extend wrote before its reader)
+  wsync();
+  if (lane == 0) apq_push(c, pid);
+  wsync();
+}
+DCU_NOINL int fp_extend(Ctx& c, int& nfp, int P, int s, int lane) {      // extendPath (:3989-4056); P == -1 -> empty path; lane 0 writes the record
   const WS w = c.ws;
   int ppos = P < 0 ? 0 : w.fp_pos()[P], plen = P < 0 ? 0 : w.fp_len()[P];
-  int o = sfo_fwd(c, s, ppos);
+  int o = sfo_fwd(c, s, ppos, lane);
   int L = w.ds_len()[s];
   double wt; int bl;
   if (plen == 0) { bl = L + c.k - 1; wt = o >= 0 ? w.sfs()[o].w : 0.0; }
@@ -1497,67 +1555,74 @@ DCU_NOINL int fp_extend(Ctx& c, int& nfp, int P, int s) {         // extendPath 
   DCU_PEAK(10, nfp + 1);
   if (nfp >= DCU_CAP.FP) { c.overflow = 14; return -1; }
   int id = nfp++;
-  w.fp_w()[id] = wt; w.fp_parent()[id] = P < 0 ? IDX_NONE : (uint32_t)P; w.fp_stretch()[id] = (uint16_t)s;
-  w.fp_pos()[id] = (uint16_t)(ppos + L - 1); w.fp_len()[id] = (uint16_t)(plen + 1); w.fp_baselen()[id] = (uint16_t)bl;
+  if (lane == 0) {
+    w.fp_w()[id] = wt; w.fp_parent()[id] = P < 0 ? IDX_NONE : (uint32_t)P; w.fp_stretch()[id] = (uint16_t)s;
+    w.fp_pos()[id] = (uint16_t)(ppos + L - 1); w.fp_len()[id] = (uint16_t)(plen + 1); w.fp_baselen()[id] = (uint16_t)bl;
+  }
   return id;
 }
-// appends the symbols 1..L-1 of a stretch as ASCII (codes -> "ACGT" by shifts); four symbols are requested before the first is used.
-// Returns the new length or -1 when the candidate buffer is full.
-DCU_FN int decode_syms(const uint8_t* sym, int L, uint8_t* out, int o) {
-  if (o + (L > 1 ? L - 1 : 0) > MAXCAND) return -1;
-  int j = 1;
+// writes the symbols 1..L-1 of a stretch as ASCII (codes -> "ACGT" by shifts) to out[o ..]: lanes over symbols
+DCU_FN void decode_syms(const uint8_t* sym, int L, uint8_t* out, int o, int lane) {
   DCU_NOUNROLL
-  for (; j + 4 <= L; j += 4) {
-    const uint32_t s0 = sym[j], s1 = sym[j + 1], s2 = sym[j + 2], s3 = sym[j + 3];
-    out[o] = (uint8_t)(0x54474341u >> (8 * s0)); out[o + 1] = (uint8_t)(0x54474341u >> (8 * s1)); out[o + 2] = (uint8_t)(0x54474341u >> (8 * s2)); out[o + 3] = (uint8_t)(0x54474341u >> (8 * s3));
-    o += 4;
-  }
-  DCU_NOUNROLL
-  for (; j < L; ++j) out[o++] = (uint8_t)(0x54474341u >> (8 * (uint32_t)sym[j]));
-  return o;
+  for (int j = 1 + lane; j < L; j += DCU_NL) out[o + j - 1] = (uint8_t)(0x54474341u >> (8 * (uint32_t)sym[j]));
 }
-// decodePathPair (:4267-4300) into ASCII; returns length or -1
-DCU_BIG int decode_pair(const Ctx& c, int P, int rpid, uint8_t* out) {
+// decodePathPair (:4267-4300) into ASCII; returns length or -1 (more than MAXCAND stretches or bases).  All lanes walk the two parent
+// chains; the symbols of a stretch are written by the lanes.  A forward path needs no stack of its stretches: fp_pos of a path is the
+// number of symbols behind the first k-mer up to and including its last stretch, so every stretch knows where its symbols go.
+DCU_BIG int decode_pair(const Ctx& c, int P, int rpid, uint8_t* out, int lane) {
   const WS w = c.ws;
-  int stack[MAXCAND]; int sp = 0;
+  if ((int)w.fp_len()[P] > MAXCAND) return -1;
+  int o = c.k + (int)w.fp_pos()[P];
+  if (o > MAXCAND) return -1;
+  int s = 0;
   DCU_NOUNROLL
-  for (int q = P; q >= 0; q = (w.fp_parent()[q] == IDX_NONE ? -1 : (int)w.fp_parent()[q])) { if (sp >= MAXCAND) return -1; stack[sp++] = w.fp_stretch()[q]; }
-  int o = 0;
-  uint32_t fk = w.n_kmer()[ds_first(c, stack[sp - 1])];
-  DCU_NOUNROLL
-  for (int i = 0; i < c.k; ++i) { if (o >= MAXCAND) return -1; out[o++] = "ACGT"[(fk >> (2 * (c.k - 1 - i))) & 3]; }
-  DCU_NOUNROLL
-  for (int t = sp - 1; t >= 0; --t) {
-    int s = stack[t], off = w.ds_off()[s], L = w.ds_len()[s];
-    o = decode_syms(w.slsym() + off, L, out, o);
-    if (o < 0) return -1;
+  for (int q = P; q >= 0; q = (w.fp_parent()[q] == IDX_NONE ? -1 : (int)w.fp_parent()[q])) {
+    s = w.fp_stretch()[q];
+    const int L = w.ds_len()[s];
+    decode_syms(w.slsym() + w.ds_off()[s], L, out, c.k + (int)w.fp_pos()[q] - (L - 1), lane);
   }
+  const uint32_t fk = w.n_kmer()[ds_first(c, s)];      // s: the first stretch of the path
+  DCU_NOUNROLL
+  for (int i = lane; i < c.k; i += DCU_NL) out[i] = (uint8_t)(0x54474341u >> (8 * ((fk >> (2 * (c.k - 1 - i))) & 3u)));
   DCU_NOUNROLL
   for (int q = rpid; w.rp_len()[q] > 0; q = (int)w.rp_parent()[q]) {
-    int s = w.rp_stretch()[q], off = w.ds_off()[s], L = w.ds_len()[s];
-    o = decode_syms(w.slsym() + off, L, out, o);
-    if (o < 0) return -1;
+    s = w.rp_stretch()[q];
+    const int L = w.ds_len()[s];
+    if (o + (L > 1 ? L - 1 : 0) > MAXCAND) return -1;
+    decode_syms(w.slsym() + w.ds_off()[s], L, out, o, lane);
+    o += L > 1 ? L - 1 : 0;
   }
   return o;
 }
 
-// forward search + pair enumeration for one (first,last) pair (:4826-5092); lane 0
-DCU_BIG void search_pair(Ctx& c, int Fnode, int lmin, int lmax, int narp, int& ncdh, uint32_t& freeslots) {
+// forward search + pair enumeration for one (first,last) pair (:4826-5092)
+DCU_BIG void search_pair(Ctx& c, int Fnode, int lmin, int lmax, int narp, int& ncdh, uint32_t& freeslots, int lane) {
   const WS& w = c.ws;
   int nfp = 0, nsi = 0, nsq = 0;
   const int K = c.k;
   DCU_NOUNROLL
-  for (int i = 0; i < DCU_CAP.BL; ++i) w.apq_n()[i] = 0;
+  for (int i = lane; i < DCU_CAP.BL; i += DCU_NL) w.apq_n()[i] = 0;
   if (w.n_dsf()[Fnode] != NID_NONE)
     DCU_NOUNROLL
-    for (int s = w.n_dsf()[Fnode], se = s + w.n_dsn()[Fnode]; s < se; ++s) { int id = fp_extend(c, nfp, -1, s); if (id < 0) return; apq_push(c, id); }
+    for (int s = w.n_dsf()[Fnode], se = s + w.n_dsn()[Fnode]; s < se; ++s) { int id = fp_extend(c, nfp, -1, s, lane); if (id < 0) return; apq_push_l0(c, id, lane); }
+  wsync();                                             // the counts are zero for every lane (a first k-mer without a stretch pushes nothing, and so syncs nothing)
+  int zz = 0;
   DCU_NOUNROLL
-  for (int zz = 0; zz < DCU_CAP.BL && !c.overflow; ++zz) {
-    DCU_NOUNROLL
-    while (w.apq_n()[zz] > 0) {
+  while (!c.overflow) {
+    // the shortest length from zz on that has a path waiting (a push goes to the length being served or to a longer one): lanes over lengths
+    {
+      uint32_t hb = 0; int base = zz;
+      DCU_NOUNROLL
+      for (; base < DCU_CAP.BL; base += DCU_NL) { const int i = base + lane; hb = ballot(i < DCU_CAP.BL && w.apq_n()[i] > 0); if (hb) break; }
+      if (!hb) break;
+      zz = base + popc((hb - 1u) & ~hb);
+    }
+    {
       double* hw = w.apq_w() + zz * HEAPK; uint32_t* hi = w.apq_id() + zz * HEAPK; int n = w.apq_n()[zz];
       int P = (int)hi[0];
-      heap_pop(false, hw, hi, n); w.apq_n()[zz] = (uint8_t)n;
+      wsync();
+      if (lane == 0) { heap_pop(false, hw, hi, n); w.apq_n()[zz] = (uint8_t)n; }
+      wsync();                                         // a path that neither pairs nor extends passes no other sync before the counts are scanned again
       int candlen = w.fp_pos()[P] + K;
       int pls = w.fp_stretch()[P];
       int plast = ds_last(c, pls); uint32_t plk = w.n_kmer()[plast];
@@ -1568,36 +1633,37 @@ DCU_BIG void search_pair(Ctx& c, int Fnode, int lmin, int lmax, int narp, int& n
       if (blo <= 255) {
         const unsigned long long* ak = w.arp_k();
         const unsigned long long klo = ((unsigned long long)plk << 8) | (unsigned long long)blo, khi = ((unsigned long long)plk << 8) | (unsigned long long)(bhi > 255 ? 255 : bhi);
-        int a = 0, b = narp;                           // first i with ak[i] >= klo
+        int a = 0, e = 0;                              // the keys ascend: first i with ak[i] >= klo = number of keys below klo; first i with ak[i] > khi likewise
         DCU_NOUNROLL
-        while (a < b) { int mid = (a + b) >> 1; if (ak[mid] < klo) a = mid + 1; else b = mid; }
-        int e = a, f = narp;                           // first i with ak[i] > khi
-        DCU_NOUNROLL
-        while (e < f) { int mid = (e + f) >> 1; if (ak[mid] <= khi) e = mid + 1; else f = mid; }
+        for (int base = 0; base < narp; base += DCU_NL) {
+          const int i = base + lane;
+          const unsigned long long kv = i < narp ? ak[i] : ~0ull;
+          a += popc(ballot(i < narp && kv < klo)); e += popc(ballot(i < narp && kv <= khi));
+        }
         if (e > a) { left = a; right = e; }
       }
       if (left >= 0) {
-        int cur = interval_next(c, left, right, -1);
+        int cur = interval_next(c, left, right, -1, lane);
         DCU_PEAK(11, nsi + 1);
         if (nsi >= DCU_CAP.SI || nsq >= DCU_CAP.SI) { c.overflow = 15; return; }
         int rec = nsi++;
-        w.si_left()[rec] = (uint16_t)left; w.si_right()[rec] = (uint16_t)right; w.si_cur()[rec] = (uint16_t)cur; w.si_path()[rec] = (uint32_t)P;
-        w.si_w()[rec] = pair_score(c, P, (int)w.arp()[cur]);
-        heap_push(true, w.sq_w(), w.sq_id(), nsq, w.si_w()[rec], (uint32_t)rec);
+        const double sc = pair_score(c, P, (int)w.arp()[cur], lane);
+        if (lane == 0) { w.si_left()[rec] = (uint16_t)left; w.si_right()[rec] = (uint16_t)right; w.si_cur()[rec] = (uint16_t)cur; w.si_path()[rec] = (uint32_t)P; w.si_w()[rec] = sc; }
+        heap_push_l0(true, w.sq_w(), w.sq_id(), nsq, sc, (uint32_t)rec, lane);
       }
       int pbl = w.fp_baselen()[P];
       if (pbl < K || (pbl - K) < ((lmax + 1) / 2)) {
         DCU_NOUNROLL
         for (int s = w.n_dsf()[plast], se = (s == NID_NONE ? 0 : s + w.n_dsn()[plast]); s < se; ++s) {
-          int o = sfo_fwd(c, s, w.fp_pos()[P]);
+          int o = sfo_fwd(c, s, w.fp_pos()[P], lane);
           double ew = o >= 0 ? w.sfs()[o].w : 0.0;
           if (ew > 0.1) {
             int L = w.ds_len()[s];
             double nwt = w.fp_w()[P] + (w.sfs()[o].w - w.sfs()[o].wf);
             if (nwt > 0.1 && (w.fp_pos()[P] + L - 1 + K) <= lmax) {
-              int id = fp_extend(c, nfp, P, s);
+              int id = fp_extend(c, nfp, P, s, lane);
               if (id < 0) return;
-              apq_push(c, id);
+              apq_push_l0(c, id, lane);
             }
           }
         }
@@ -1608,31 +1674,37 @@ DCU_BIG void search_pair(Ctx& c, int Fnode, int lmin, int lmax, int narp, int& n
   DCU_NOUNROLL
   for (int nfull = 0; nsq > 0 && nfull < 16 && !c.overflow; ++nfull) {        // :5049-5092
     int rec = (int)w.sq_id()[0]; double weight = w.sq_w()[0];
-    heap_pop(true, w.sq_w(), w.sq_id(), nsq);
+    heap_pop_l0(true, w.sq_w(), w.sq_id(), nsq, lane);
     int P = (int)w.si_path()[rec], cur = w.si_cur()[rec];
-    int nxt = interval_next(c, w.si_left()[rec], w.si_right()[rec], cur);
+    int nxt = interval_next(c, w.si_left()[rec], w.si_right()[rec], cur, lane);
     if (nxt >= 0) {
       if (nsi >= DCU_CAP.SI) { c.overflow = 16; return; }
       int r2 = nsi++;
-      w.si_left()[r2] = w.si_left()[rec]; w.si_right()[r2] = w.si_right()[rec]; w.si_cur()[r2] = (uint16_t)nxt; w.si_path()[r2] = (uint32_t)P;
-      w.si_w()[r2] = pair_score(c, P, (int)w.arp()[nxt]);
-      heap_push(true, w.sq_w(), w.sq_id(), nsq, w.si_w()[r2], (uint32_t)r2);
+      const double sc = pair_score(c, P, (int)w.arp()[nxt], lane);
+      if (lane == 0) { w.si_left()[r2] = w.si_left()[rec]; w.si_right()[r2] = w.si_right()[rec]; w.si_cur()[r2] = (uint16_t)nxt; w.si_path()[r2] = (uint32_t)P; w.si_w()[r2] = sc; }
+      heap_push_l0(true, w.sq_w(), w.sq_id(), nsq, sc, (uint32_t)r2, lane);
     }
     if (ncdh == CDH_N) {
       if (weight <= w.cdh_w()[0]) continue;
       freeslots |= 1u << w.cdh_id()[0];
-      heap_pop(false, w.cdh_w(), w.cdh_id(), ncdh);
+      heap_pop_l0(false, w.cdh_w(), w.cdh_id(), ncdh, lane);
     }
-    int len = decode_pair(c, P, (int)w.arp()[cur], w.tmps());
+    const int len = decode_pair(c, P, (int)w.arp()[cur], w.tmps(), lane);
     if (len < 0) { c.overflow = 17; return; }
-    if (len == prevlen) { bool eq = true; for (int i = 0; i < len; ++i) if (w.tmps()[i] != w.prevs()[i]) { eq = false; break; } if (eq) continue; }
+    wsync();
+    if (len == prevlen) {                              // the candidate just emitted again: lanes over its bases
+      bool ne = false;
+      DCU_NOUNROLL
+      for (int i = lane; i < len; i += DCU_NL) ne = ne || w.tmps()[i] != w.prevs()[i];
+      if (!ballot(ne)) continue;
+    }
     prevlen = len;
     int slot = 0; while (!((freeslots >> slot) & 1u)) ++slot;
     freeslots &= ~(1u << slot);
     DCU_NOUNROLL
-    for (int i = 0; i < len; ++i) { w.prevs()[i] = w.tmps()[i]; w.cand()[slot * MAXCAND + i] = w.tmps()[i]; }
-    w.candlen()[slot] = (uint8_t)len;
-    heap_push(false, w.cdh_w(), w.cdh_id(), ncdh, weight, (uint32_t)slot);
+    for (int i = lane; i < len; i += DCU_NL) { const uint8_t ch = w.tmps()[i]; w.prevs()[i] = ch; w.cand()[slot * MAXCAND + i] = ch; }      // (a lane compares and rewrites the same bases of prevs)
+    if (lane == 0) w.candlen()[slot] = (uint8_t)len;
+    heap_push_l0(false, w.cdh_w(), w.cdh_id(), ncdh, weight, (uint32_t)slot, lane);
   }
 }
 
@@ -1670,7 +1742,7 @@ DCU_BIG bool trav_seek(Ctx& c, TravState& t) {
   }
 }
 // one (first,last) pair at (fi, li), then advances li  (:4802-5097), in two halves so that the kernel can put a barrier between
-// the lane-parallel graph work (trav_pair_graph) and the single-lane searches (trav_pair_search)
+// the graph work (trav_pair_graph) and the searches (trav_pair_search)
 DCU_BIG void trav_pair_graph(Ctx& c, TravState& t, int lane) {
   const WS w = c.ws;
   c.epoch_pair = ++c.epoch;
@@ -1696,7 +1768,7 @@ DCU_BIG void trav_pair_weights(Ctx& c, int lane) {
 }
 DCU_BIG void trav_pair_rpaths(Ctx& c, TravState& t, int lmax, int lane) {
   int narp = 0;
-  // stretches whose last k-mer is L, in index order (all lanes; the seed of the reverse search used to scan all stretches on lane 0)
+  // stretches whose last k-mer is L, in index order
   const WS w = c.ws;
   int nseed = 0;
   DCU_NOUNROLL
@@ -1708,8 +1780,7 @@ DCU_BIG void trav_pair_rpaths(Ctx& c, TravState& t, int lmax, int lane) {
     nseed += popc(hb);
   }
   wsync();
-  if (lane == 0) reverse_paths(c, t.L, lmax, narp, nseed);
-  c.overflow = bcast(c.overflow, 0); narp = bcast(narp, 0);
+  reverse_paths(c, t.L, lmax, narp, nseed, lane);
   wsync();
   t.narp = narp;
   if (c.overflow) return;
@@ -1723,9 +1794,8 @@ DCU_BIG void trav_pair_search(Ctx& c, TravState& t, int lmin, int lmax, int lane
 #ifdef DCU_EMU_STATS
   const int ncdh_before = t.ncdh; const uint32_t fs_before = t.freeslots;
 #endif
-  if (lane == 0) search_pair(c, t.F, lmin, lmax, t.narp, ncdh, fs);
-  t.ncdh = bcast(ncdh, 0); t.freeslots = bcast(fs, 0);
-  c.overflow = bcast(c.overflow, 0);
+  search_pair(c, t.F, lmin, lmax, t.narp, ncdh, fs, lane);
+  t.ncdh = ncdh; t.freeslots = fs;
   wsync();
 #ifdef DCU_EMU_STATS
   g_stats[8] += (t.ncdh == ncdh_before && t.freeslots == fs_before);      // pairs that left the candidate heap untouched
