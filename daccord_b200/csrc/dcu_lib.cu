@@ -15,6 +15,18 @@
 #include <map>
 #include <tuple>
 #include <chrono>
+// Per-stage clocks of the window kernels (-DDCU_STAGE_CLOCKS, a measurement build next to the product library, read by
+// tools/stage_clocks.py): clock64() around every stage call and every group barrier, summed per warp in shared memory and added to
+// g_stage_clk when the warp leaves the kernel.  clock64() is per SM: only differences taken by one warp are summed.  Without the
+// switch the macros expand to the bare statement and the kernels are the product's, instruction for instruction.
+// Slots: busy cycles of the nine stages, their calls, wait cycles at the round barrier (slot CLK_WAIT) and at the barrier behind each of
+// the first eight stages, fetch (ticket, st_begin, publish), barrier waits of a warp that has no window left, the warp's whole life;
+// then busy cycles and calls of three parts of the pos stage (raw-unitig fill, split-piece fill, stretch_links), which window_core.cuh
+// adds to g_stage_clk directly (DCU_POS_CLK): they are declared here, ahead of it.
+#ifdef DCU_STAGE_CLOCKS
+enum { CLK_BUSY = 0, CLK_CALLS = 9, CLK_WAIT = 18, CLK_FETCH = 27, CLK_IDLE = 28, CLK_LIFE = 29, CLK_POS = 30, CLK_N = 36 };
+__device__ unsigned long long g_stage_clk[CLK_N];
+#endif
 #include "window_core.cuh"            // namespace dcu : every workspace field in the warp's HBM slab (overflow passes, deep piles)
 #define DCU_NS dcus
 #define DCU_TIER_SMEM 1
@@ -60,21 +72,14 @@ struct KArgs {
   unsigned int launch_seq;             // number of this launch in the context's life (upper half of the forward slot tags: records of earlier launches in the slab are stale)
 };
 
-// Per-stage clocks of the window kernels (-DDCU_STAGE_CLOCKS, a measurement build next to the product library, read by
-// tools/stage_clocks.py): clock64() around every stage call and every group barrier, summed per warp in shared memory and added to
-// g_stage_clk when the warp leaves the kernel.  clock64() is per SM: only differences taken by one warp are summed.  Without the
-// switch the macros expand to the bare statement and the kernels are the product's, instruction for instruction.
-// Slots: busy cycles of the nine stages, their calls, wait cycles at the round barrier (slot CLK_WAIT) and at the barrier behind each of
-// the first eight stages, fetch (ticket, st_begin, publish), barrier waits of a warp that has no window left, the warp's whole life.
+// (the per-stage clocks: see the top of the file)
 #ifdef DCU_STAGE_CLOCKS
-enum { CLK_BUSY = 0, CLK_CALLS = 9, CLK_WAIT = 18, CLK_FETCH = 27, CLK_IDLE = 28, CLK_LIFE = 29, CLK_N = 30 };
-__device__ unsigned long long g_stage_clk[CLK_N];
-#define DCU_CLK_DECL(NW) __shared__ unsigned long long s_clk[NW][CLK_N]; if (lane == 0) for (int i_ = 0; i_ < CLK_N; ++i_) s_clk[warp][i_] = 0; const long long clk_life_ = clock64();
+#define DCU_CLK_DECL(NW) __shared__ unsigned long long s_clk[NW][CLK_POS]; if (lane == 0) for (int i_ = 0; i_ < CLK_POS; ++i_) s_clk[warp][i_] = 0; const long long clk_life_ = clock64();
 #define DCU_CLK_STAGE(i, call) do { const long long t0_ = clock64(); call; if (lane == 0) { s_clk[warp][CLK_BUSY + (i)] += (unsigned long long)(clock64() - t0_); s_clk[warp][CLK_CALLS + (i)] += 1; } } while (0)
 #define DCU_CLK_WAIT(i, call) do { const long long t0_ = clock64(); call; if (lane == 0) s_clk[warp][idle ? (int)CLK_IDLE : CLK_WAIT + (i)] += (unsigned long long)(clock64() - t0_); } while (0)
 #define DCU_CLK_FETCH_BEGIN const long long clk_f0_ = clock64();
 #define DCU_CLK_FETCH_END if (lane == 0) s_clk[warp][CLK_FETCH] += (unsigned long long)(clock64() - clk_f0_);
-#define DCU_CLK_FLUSH if (lane == 0) { s_clk[warp][CLK_LIFE] = (unsigned long long)(clock64() - clk_life_); for (int i_ = 0; i_ < CLK_N; ++i_) atomicAdd(&g_stage_clk[i_], s_clk[warp][i_]); }
+#define DCU_CLK_FLUSH if (lane == 0) { s_clk[warp][CLK_LIFE] = (unsigned long long)(clock64() - clk_life_); for (int i_ = 0; i_ < CLK_POS; ++i_) atomicAdd(&g_stage_clk[i_], s_clk[warp][i_]); }
 #else
 #define DCU_CLK_DECL(NW)
 #define DCU_CLK_STAGE(i, call) call

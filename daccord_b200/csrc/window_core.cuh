@@ -41,6 +41,19 @@
 #ifndef DCU_WIDE
 #define DCU_WIDE 0
 #endif
+// clock build of the library (dcu_lib.cu, -DDCU_STAGE_CLOCKS): busy cycles and calls of part i of the pos stage, added by lane 0 to the
+// slots CLK_POS + i / CLK_POS + 3 + i of g_stage_clk (declared by dcu_lib.cu); otherwise the bare statement
+#ifndef DCU_POS_CLK
+#if defined(DCU_STAGE_CLOCKS) && !defined(DCU_EMU)
+#define DCU_POS_CLK(i, ...)                                                                                                            \
+  do {                                                                                                                                 \
+    const long long t0_ = clock64(); __VA_ARGS__;                                                                                      \
+    if (lane == 0) { atomicAdd(&g_stage_clk[CLK_POS + (i)], (unsigned long long)(clock64() - t0_)); atomicAdd(&g_stage_clk[CLK_POS + 3 + (i)], 1ull); } \
+  } while (0)
+#else
+#define DCU_POS_CLK(i, ...) __VA_ARGS__
+#endif
+#endif
 
 namespace DCU_NS {
 using namespace dcub;
@@ -1063,7 +1076,7 @@ template <bool SM> DCU_FN const uint8_t* vs_col(const Ctx& c, int p) {
   return (const uint8_t*)c.vsq + (uint32_t)p * 8u;
 }
 // positional weight sum of one node at one true position p (this lane's): sum over the instance list ip[0,f) of VS[min(ip[t],MS)][p].
-// Every lane walks the list itself (all lanes of a warp read the same instance byte: a broadcast load), no shuffles in the loop.
+// Every lane walks its list itself, no shuffles in the loop (lanes on the same node read the same instance byte: a broadcast load).
 template <bool SM> DCU_FN unsigned long long inst_colsum(const Ctx& c, const uint8_t* ip, int f, int p, int NP, int MS) {
   unsigned long long u = 0;
   const uint32_t row = (uint32_t)NP * 8u;
@@ -1086,49 +1099,66 @@ template <bool SM> DCU_FN unsigned long long inst_colsum(const Ctx& c, const uin
 // support range (forward: first k-mer, object p = start position; reverse: last k-mer, object p = its reverse
 // position); slot weight < 0 marks "not feasible".  A slot holds the sum of the link weights and the weight of the first (forward: also of
 // the last) link (StretchFeasObject::wf / wl, :875-889), so that the searches never evaluate a node weight themselves.
-// The REVERSE slots are all needed (stretch_links combines them pairwise) and are filled here, by sp_view.  The FORWARD slots are only ever
+// The REVERSE slots are all needed (stretch_links combines them pairwise) and are filled here, by rev_fill.  The FORWARD slots are only ever
 // read by the forward search, which looks at a few per cent of them (tools/field_traffic.py: 1 050 slots written, 40 read per window):
 // they are evaluated on demand by the search itself (fwd_slot_eval) and remembered in the slot record, tagged with the traverse / pair
 // they belong to.  Same arithmetic in the same order either way.
-// sp_view fills the reverse slots of one view (off, L) of the link array: lanes over anchor positions; the link weights are evaluated
-// from the instance lists (all lanes share the node, so instance positions are uniform loads and only the table column differs per
-// lane).  Warp-uniform arguments.  The descriptors of up to 32 links are fetched at once, lane t taking link j0 + t, and the loop gets
-// them by shuffle.
-template <bool SM> DCU_FN void sp_view_t(const Ctx& c, int off, int L, int nr, int br, uint32_t cO, int lane) {
+// rev_fill fills the reverse slots [s0, s1) of nv views (offset, length) of the link array whose slot ranges tile [s0, s1) in view
+// order: view v (unitig u = ids[v], or v without ids) owns the slots from vcO[u] on, one per reverse position of its last k-mer.  Lanes
+// go over slots, across views, so that the warp is full however few positions a unitig has (17 on average at 40x, 15 at 10x).  A lane
+// finds its view among the 32 that follow the previous group's last one (lane t loads the first slot of one of them, a search by
+// shuffles over these ascending offsets), by a binary search over the offsets only when more than 32 views start in one group.  It
+// then walks the view's links in order itself, the descriptor of the next link in flight while the current one is weighed: the sum of
+// the link weights is the one a single lane makes, and a slot stops at its first failing link, so no link is weighed in vain.
+// Warp-uniform arguments.
+template <bool SM> DCU_FN void rev_fill_t(const Ctx& c, const uint16_t* voff, const uint16_t* vlen, const uint32_t* vcO, const uint16_t* ids,
+                                          int nv, uint32_t s0, uint32_t s1, int lane) {
   const WS w = c.ws;
   const int NP = DCU_T.NP, MS = DCU_T.MS;
+  int lo = 0;                                          // the view of the group's first slot
   DCU_NOUNROLL
-  for (int q0 = 0; q0 < nr; q0 += DCU_NL) {
-    const int q = q0 + lane;
-    bool ar = q < nr;
-    double sumr = 0.0, wfr = 0.0;
+  for (uint32_t g = s0; g < s1; g += DCU_NL) {
+    const uint32_t o = g + lane;
+    const int vt = lo + 1 + lane;
+    const uint32_t st = vt < nv ? vcO[ids ? ids[vt] : vt] : 0xFFFFFFFFu;
+    int k = 0;                                         // k = number of the views lo + 1 .. lo + 32 whose first slot is <= o
     DCU_NOUNROLL
-    for (int j0 = 0; j0 < L; j0 += DCU_NL) {
-      // descriptors of the links j0 .. j0 + 31 of the reverse walk: lane t holds the node of link L - 1 - (j0 + t)
-      uint32_t dioR = 0; int dfR = 0;
-      if (j0 + lane < L) { const int nR = w.slinks()[off + L - 1 - (j0 + lane)]; dioR = w.n_ioff()[nR]; dfR = w.n_freq()[nR]; }
-      const int jn = L - j0 < DCU_NL ? L - j0 : DCU_NL;
-      if (!ballot(ar)) break;                          // nothing feasible left in this group of positions (checked once per 32 links)
-      DCU_NOUNROLL
-      for (int t = 0; t < jn; ++t) {
-        const int jj = j0 + t;
-        const uint32_t ioR = bcast(dioR, t); const int fR = bcast(dfR, t);
-        if (ar) {                                      // link L-1-jj at reverse position br + q + jj
-          const int p = br + q + jj;
-          double wt = 0.0;
-          if (p < NP) wt = (double)inst_colsum<SM>(c, w.irpos() + ioR, fR, p, NP, MS) * 2.3283064365386963e-10;
-          if (wt >= 1e-3) { sumr += wt; if (jj == 0) wfr = wt; } else ar = false;
-        }
+    for (int h = DCU_NL / 2; h > 0; h >>= 1) if (bcast(st, k + h - 1) <= o) k += h;
+    if (bcast(st, DCU_NL - 1) <= o) k = DCU_NL;
+    int v = lo + k;
+    if (o < s1) {
+      if (k == DCU_NL) {                               // the last view whose first slot is <= o
+        int hi = nv;
+        DCU_NOUNROLL
+        while (hi - v > 1) { const int mid = (v + hi) >> 1; if (vcO[ids ? ids[mid] : mid] <= o) v = mid; else hi = mid; }
       }
-    }
-    if (q < nr) { RSlot r; r.w = ar ? sumr : -1.0; r.wf = wfr; w.scs()[cO + q] = r; }
+      const int u = ids ? ids[v] : v;
+      const int off = voff[u], L = vlen[u], q = (int)(o - vcO[u]);
+      const int n0 = w.slinks()[off + L - 1];          // link 0 of the reverse walk: the last k-mer, whose reverse range starts at br
+      const int br = w.n_cpf()[n0];
+      uint32_t io = w.n_ioff()[n0]; int f = w.n_freq()[n0];
+      double sum = 0.0, wf = 0.0; bool ok = true;
+      DCU_NOUNROLL
+      for (int j = 0; j < L; ++j) {                    // link L-1-j at reverse position br + q + j
+        uint32_t io1 = 0; int f1 = 0;
+        if (j + 1 < L) { const int n1 = w.slinks()[off + L - 2 - j]; io1 = w.n_ioff()[n1]; f1 = w.n_freq()[n1]; }
+        const int p = br + q + j;
+        double wt = 0.0;
+        if (p < NP) wt = (double)inst_colsum<SM>(c, w.irpos() + io, f, p, NP, MS) * 2.3283064365386963e-10;
+        if (!(wt >= 1e-3)) { ok = false; break; }
+        sum += wt; if (j == 0) wf = wt;
+        io = io1; f = f1;
+      }
+      RSlot r; r.w = ok ? sum : -1.0; r.wf = wf; w.scs()[o] = r;
+    } else v = lo;
+    lo = bcast(v, DCU_NL - 1);
   }
 }
-DCU_NOINL void sp_view(const Ctx& c, int off, int L, int nr, int br, uint32_t cO, int lane) {
+DCU_NOINL void rev_fill(const Ctx& c, const uint16_t* voff, const uint16_t* vlen, const uint32_t* vcO, const uint16_t* ids, int nv, uint32_t s0, uint32_t s1, int lane) {
 #ifndef DCU_EMU
-  if (c.vs_sm) { sp_view_t<true>(c, off, L, nr, br, cO, lane); return; }
+  if (c.vs_sm) { rev_fill_t<true>(c, voff, vlen, vcO, ids, nv, s0, s1, lane); return; }
 #endif
-  sp_view_t<false>(c, off, L, nr, br, cO, lane);
+  rev_fill_t<false>(c, voff, vlen, vcO, ids, nv, s0, s1, lane);
 }
 // one forward slot: stretch s anchored at true position p (the forward search calls this the first time it looks at a slot).  Warp-uniform
 // arguments, every lane returns the record.  The links are taken 32 at a time; when fewer are left, G lanes share a link (unitigs are short:
@@ -1207,14 +1237,7 @@ DCU_BIG void stretch_positions(Ctx& c, int lane) {
       wsync();
       DCU_PEAK(6, run0 > run1 ? run0 : run1);
       if (run0 > (uint32_t)DCU_CAP.SF || run1 > (uint32_t)DCU_CAP.SF) { c.overflow = 9; return; }
-      DCU_NOUNROLL
-      for (int r = 0; r < c.nrs; ++r) {
-        const int off = w.rs_off()[r], L = w.rs_len()[r];
-        const int n1 = w.slinks()[off + L - 1];
-        const int br = w.n_cpf()[n1];
-        const int nr = (uint8_t)(w.n_cpt()[n1] - br);
-        sp_view(c, off, L, nr, br, w.rs_cO()[r], lane);
-      }
+      DCU_POS_CLK(0, rev_fill(c, w.rs_off(), w.rs_len(), w.rs_cO(), nullptr, c.nrs, 0, run1, lane));
       if (lane == 0) { w.spc()[0] = 1; w.spc()[1] = run0; w.spc()[2] = run1; }
       wsync();
     }
@@ -1253,11 +1276,7 @@ DCU_BIG void stretch_positions(Ctx& c, int lane) {
   wsync();
   DCU_PEAK(6, run0 > run1 ? run0 : run1);
   if (run0 > (uint32_t)DCU_CAP.SF || run1 > (uint32_t)DCU_CAP.SF) { c.overflow = 9; return; }
-  DCU_NOUNROLL
-  for (int t = 0; t < ntodo; ++t) {
-    const int s = todo[t];
-    sp_view(c, w.ds_off()[s], w.ds_len()[s], w.ds_cN()[s], w.ds_cB()[s], w.ds_cO()[s], lane);
-  }
+  DCU_POS_CLK(1, rev_fill(c, w.ds_off(), w.ds_len(), w.ds_cO(), todo, ntodo, base1, run1, lane));
   wsync();
 }
 // getCachedStretchPositionWeight (:3906-3918); evaluates the slot at its first use.  Warp-uniform: all lanes look at the record, the warp
@@ -1282,32 +1301,43 @@ DCU_NOINL int sfo_rev(const Ctx& c, int s, int p) {     // getCachedStretchRever
 // (the weights of the first / last link of a stretch object, StretchFeasObject::wf / wl :875-889, are fields of the slot records)
 
 // computeStretchLinks / getReverseStretchLinkWeight (:3388-3480): link A -> B (B.first == A.last) kept iff
-// max over common reverse positions of w_B + (w_A - wf_A) >= 0.1; stored as (B,A), sorted; lanes over A
+// max over common reverse positions of w_B + (w_A - wf_A) >= 0.1; stored as (B,A), sorted.  The test is that some common position has
+// w_B + (w_A - wf_A) >= 0.1 (the maximum is exact and starts at 0): a pair stops at its first such position.  Lanes go over the (A, B)
+// pairs of a group of 32 stretches A (each A has at most four B): a lane finds the A of its pair by a binary search over the lanes'
+// inclusive pair counts.  The keys are appended by atomics in any order and sorted.
 DCU_BIG void stretch_links(Ctx& c, int lane) {
   const WS w = c.ws;
   uint32_t* cnt = &w.hstate()[3];
   if (lane == 0) *cnt = 0;
   wsync();
   DCU_NOUNROLL
-  for (int A = lane; A < c.nds; A += DCU_NL) {
-    int ln = ds_last(c, A);
-    int b0 = w.n_dsf()[ln], bn = w.n_dsn()[ln];
-    if (b0 == NID_NONE) continue;
-    const int aB = w.ds_cB()[A], aN = w.ds_cN()[A]; const uint32_t aO = w.ds_cO()[A];      // A's reverse slots (what sfo_rev(A, .) looks at), loaded once
+  for (int base = 0; base < c.nds; base += DCU_NL) {
+    int b0 = 0, bn = 0;
+    if (base + lane < c.nds) { const int ln = ds_last(c, base + lane); b0 = w.n_dsf()[ln]; bn = b0 == NID_NONE ? 0 : w.n_dsn()[ln]; }
+    const uint32_t e = scan_incl((uint32_t)bn, lane);
+    const int np = (int)bcast(e, DCU_NL - 1);
     DCU_NOUNROLL
-    for (int B = b0; B < b0 + bn; ++B) {
-      int shift = w.ds_len()[B] - 1;
-      double weight = 0.0;
-      int cb = w.ds_cB()[B], cn = w.ds_cN()[B], co = w.ds_cO()[B];
+    for (int t0 = 0; t0 < np; t0 += DCU_NL) {
+      const int t = t0 + lane;
+      int o = 0;                                       // the first lane whose inclusive count exceeds t
       DCU_NOUNROLL
-      for (int d = 0; d < cn; ++d) {
+      for (int h = DCU_NL / 2; h > 0; h >>= 1) if ((int)bcast(e, o + h - 1) <= t) o += h;
+      const int ob0 = bcast(b0, o), obn = bcast(bn, o), oe = (int)bcast(e, o);
+      if (t >= np) continue;
+      const int A = base + o, B = ob0 + t - (oe - obn);
+      const int aB = w.ds_cB()[A], aN = w.ds_cN()[A]; const uint32_t aO = w.ds_cO()[A];      // A's reverse slots (what sfo_rev(A, .) looks at)
+      const int shift = w.ds_len()[B] - 1;
+      const int cb = w.ds_cB()[B], cn = w.ds_cN()[B], co = w.ds_cO()[B];
+      bool keep = false;
+      DCU_NOUNROLL
+      for (int d = 0; d < cn && !keep; ++d) {
         const int da = cb + d + shift - aB;
         if (da < 0 || da >= aN) continue;
         const double wb = w.scs()[co + d].w, wa = w.scs()[aO + da].w, wf = w.scs()[aO + da].wf;      // three independent loads
         if (!(wb >= 0.0) || !(wa >= 0.0)) continue;
-        const double lw = wb + (wa - wf); weight = lw > weight ? lw : weight;
+        keep = wb + (wa - wf) >= 1e-1;
       }
-      if (weight >= 1e-1) { uint32_t t = a_add(cnt, 1); if ((int)t < DCU_CAP.RL) w.rl()[t] = ((uint32_t)B << 16) | (uint32_t)A; }
+      if (keep) { uint32_t k = a_add(cnt, 1); if ((int)k < DCU_CAP.RL) w.rl()[k] = ((uint32_t)B << 16) | (uint32_t)A; }
     }
   }
   wsync();
@@ -1764,7 +1794,7 @@ DCU_BIG void trav_pair_graph(Ctx& c, TravState& t, int lane) {
 DCU_BIG void trav_pair_weights(Ctx& c, int lane) {
   stretch_positions(c, lane);
   if (c.overflow) return;
-  stretch_links(c, lane);
+  DCU_POS_CLK(2, stretch_links(c, lane));
 }
 DCU_BIG void trav_pair_rpaths(Ctx& c, TravState& t, int lmax, int lane) {
   int narp = 0;

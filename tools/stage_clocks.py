@@ -5,8 +5,9 @@ Workload of tools/ncu_target.py: windows of a simulated pile, resident in HBM.
     python tools/stage_clocks.py [Mb] [coverage] [launches] [k]      (default 20 Mb, 40x, 5 timed launches after one warm-up, k = 8)
 
 Per stage: share of all warp-cycles spent in the stage (busy), share spent waiting at the barrier that follows it, calls per window;
-then fetch (ticket, st_begin, publish), the barrier waits of warps that have no window left, and the rest (loop overhead).  The kernel
-times printed are those of the instrumented kernel (tools/ncu_target.py times the product's).  Needs a GPU; there is no fallback."""
+below pos its three parts: the reverse slots of the raw unitigs (first pair of a traverse), those of the split pieces, stretch_links
+(with its sort), and the rest of the stage (slot offsets and the capacity check); then fetch (ticket, st_begin, publish), the barrier
+waits of warps that have no window left, and the rest (loop overhead).  The kernel times printed are those of the instrumented kernel (tools/ncu_target.py times the product's).  Needs a GPU; there is no fallback."""
 import ctypes as C
 import os
 import sys
@@ -20,7 +21,8 @@ from daccord_b200.host import Dataset
 from deep_bench import card
 
 STAGES = ["hash", "nodes", "edges", "trav", "pos", "rpath", "search", "score", "final"]
-CLK_BUSY, CLK_CALLS, CLK_WAIT, CLK_FETCH, CLK_IDLE, CLK_LIFE, CLK_N = 0, 9, 18, 27, 28, 29, 30
+CLK_BUSY, CLK_CALLS, CLK_WAIT, CLK_FETCH, CLK_IDLE, CLK_LIFE, CLK_POS, CLK_N = 0, 9, 18, 27, 28, 29, 30, 36
+POS_PARTS = ["raw fill", "split fill", "links"]
 
 
 def main():
@@ -55,6 +57,10 @@ def main():
     for i, s in enumerate(STAGES):
         wait = c[CLK_WAIT + i + 1] if i < 8 else 0.0
         print("%-8s %8.2f %14.2f %14.2f" % (s, 100 * c[CLK_BUSY + i] / life, 100 * wait / life, c[CLK_CALLS + i] / nwin))
+        if s == "pos":
+            for j, part in enumerate(POS_PARTS):
+                print("  %-12s %6.2f %14s %14.2f" % (part, 100 * c[CLK_POS + j] / life, "", c[CLK_POS + 3 + j] / nwin))
+            print("  %-12s %6.2f" % ("rest", 100 * (c[CLK_BUSY + i] - c[CLK_POS:CLK_POS + 3].sum()) / life))
     acc = c[CLK_BUSY:CLK_BUSY + 9].sum() + c[CLK_WAIT:CLK_WAIT + 9].sum() + c[CLK_FETCH] + c[CLK_IDLE]
     print("%-8s %8s %14.2f" % ("round", "", 100 * c[CLK_WAIT] / life))
     print("%-8s %8.2f" % ("fetch", 100 * c[CLK_FETCH] / life))
