@@ -814,13 +814,14 @@ static int pile_impl(dcu_ctx* ctx, const dcu_overlap* ovl, uint64_t novl, const 
   dpile::Prep P;
   if (!dpile::prepare(ovl, novl, ntrace, tspace, w, advance, nreads, read_len, P, prof)) { ctx->err = P.err; return DCU_ERR_UNSUPPORTED; }
   laps.lap("prepare");
-  int bad = 0;                                   // every B block must lie inside its read and fit the tile aligner
+  int bad = 0;                                   // every B block must lie inside its read and fit the tile aligner; both reads inside the database
 #pragma omp parallel for schedule(static) reduction(max : bad)
   for (int64_t i = 0; i < (int64_t)novl; ++i) {
     uint64_t b = (uint64_t)ovl[i].bbpos; int e = 0;
     for (int32_t t = 1; t < ovl[i].tlen; t += 2) { uint16_t bl = trace[ovl[i].trace_off + t]; if (bl > dpile::PILE_MAXB) e = 3; b += bl; }
     if (b > read_len[ovl[i].bread]) e = std::max(e, 2);
-    if ((read_boff[ovl[i].bread] + (read_len[ovl[i].bread] + 3) / 4) > ctx->packed_bytes) e = std::max(e, 1);
+    for (int32_t r : {ovl[i].aread, ovl[i].bread})
+      if ((read_boff[r] + (read_len[r] + 3) / 4) > ctx->packed_bytes) e = std::max(e, 1);
     bad = std::max(bad, e);
   }
   laps.lap("validate");
