@@ -133,6 +133,23 @@ class Engine:
         self._ck(self.lib.dcu_last_profile_stats(self.ctx, C.byref(h)))
         return rec, h.value
 
+    def inqual(self, ovl, trace, tspace, read_len, first_read, last_read, depth):
+        """the intrinsic quality track of A-reads [first_read, last_read) on the GPU (dcu_inqual): ovl = every overlap of those reads in
+        .las order (daccord_b200.host.OVERLAP_DT) with their trace values; returns one uint8 per tile of tspace bases of every read, in read order"""
+        read_len = np.ascontiguousarray(read_len, np.uint32)
+        nb = int(((read_len[first_read:last_read].astype(np.uint64) + tspace - 1) // tspace).sum())
+        out = np.zeros(max(nb, 1), np.uint8)
+        n = C.c_uint64(0)
+        self._ck(self.lib.dcu_inqual(self.ctx, _p(ovl), C.c_uint64(len(ovl)), _p(trace), C.c_uint64(len(trace)), C.c_int32(tspace), _p(read_len),
+                                     C.c_uint64(first_read), C.c_uint64(last_read), C.c_uint64(depth), _p(out), C.byref(n)))
+        return out[:n.value]
+
+    def inqual_stats(self):
+        """the last inqual call: kernel time in ms (CUDA events), histogram bins, tiles per thread block (dcu_last_inqual_stats)"""
+        ms, nb, ch = C.c_float(0), C.c_uint32(0), C.c_uint32(0)
+        self._ck(self.lib.dcu_last_inqual_stats(self.ctx, C.byref(ms), C.byref(nb), C.byref(ch)))
+        return {"kernel_ms": ms.value, "bins": nb.value, "tiles_per_block": ch.value}
+
     def get_windows(self, with_slices=False):
         win = np.zeros(self.nwin, WINDOW_DT)
         sl = np.zeros(self.nsl, SLICE_DT) if with_slices else None

@@ -41,7 +41,8 @@ def build(force=False, verbose=False):
     _nvcc(LIB, [], force, verbose)
     host_src = os.path.join(csrc, "host", "hostlib.cpp")  # noqa
     host_deps = [os.path.join(csrc, "host", f) for f in os.listdir(os.path.join(csrc, "host"))] + [os.path.join(ROOT, "include", "daccord_b200.h"),
-                                                                                               os.path.join(csrc, "profile_core.cuh")]
+                                                                                               os.path.join(csrc, "profile_core.cuh"),
+                                                                                               os.path.join(csrc, "inqual_core.cuh")]
     if force or _newer(HOST_LIB, host_deps):
         subprocess.check_call(["/usr/bin/g++", "-O3", "-g", "-std=c++17", "-march=x86-64-v2", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared",
                                "-o", HOST_LIB, host_src])
@@ -49,6 +50,10 @@ def build(force=False, verbose=False):
     if force or _newer(cli, host_deps + [LIB]):
         subprocess.check_call(["/usr/bin/g++", "-O3", "-g", "-std=c++17", "-march=x86-64-v2", "-ffp-contract=off", "-fopenmp", "-pthread", "-o", cli,
                                os.path.join(csrc, "host", "daccord_main.cpp"), "-L" + BUILD, "-ldaccord_b200", "-Wl,-rpath,$ORIGIN"])
+    iqv = os.path.join(BUILD, "computeintrinsicqv")
+    if force or _newer(iqv, host_deps + [LIB]):
+        subprocess.check_call(["/usr/bin/g++", "-O3", "-g", "-std=c++17", "-march=x86-64-v2", "-ffp-contract=off", "-fopenmp", "-pthread", "-o", iqv,
+                               os.path.join(csrc, "host", "computeintrinsicqv.cpp"), "-L" + BUILD, "-ldaccord_b200", "-Wl,-rpath,$ORIGIN"])
     return LIB
 
 

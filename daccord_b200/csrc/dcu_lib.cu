@@ -42,10 +42,13 @@ __device__ unsigned long long g_stage_clk[CLK_N];
 #include "pile_host.hpp"
 #include "vote_host.hpp"
 #include "profile_core.cuh"           // namespace dprof: one window of the error-profile estimator (dcu_profile)
+#include "inqual_core.cuh"            // namespace dinq: the intrinsic quality track (dcu_inqual)
 #include "../../include/daccord_b200.h"
 
 static_assert(sizeof(dcu::Slice) == sizeof(dcu_slice) && sizeof(dcu::Window) == sizeof(dcu_window) && sizeof(dcu::Result) == sizeof(dcu_result), "ABI structs");
 static_assert(sizeof(dvote::Win) == sizeof(dcu_window) && sizeof(dvote::Res) == sizeof(dcu_result), "ABI structs (vote)");
+static_assert(sizeof(dinq::Ovl) == sizeof(dcu_overlap) && offsetof(dinq::Ovl, tlen) == offsetof(dcu_overlap, tlen) && offsetof(dinq::Ovl, trace_off) == offsetof(dcu_overlap, trace_off),
+              "ABI structs (inqual)");
 
 namespace {
 
@@ -475,6 +478,24 @@ __global__ void __launch_bounds__(PROF_TPB) prof_k(const dpile::Win* win, const 
   }
 }
 
+// ---- intrinsic quality track (inqual_core.cuh): one block per (read, chunk of P.ch tiles) -- its warps add the read's overlaps to the
+// chunk's histogram in shared memory, a warp per overlap with the lanes on consecutive tiles; then one thread per tile takes its byte
+constexpr int INQ_TPB = 256;
+__global__ void __launch_bounds__(INQ_TPB) inq_k(const dinq::Ovl* ov, const uint16_t* trace, const dinq::Read* reads, const uint2* items, int32_t tspace,
+                                                dinq::Plan P, uint64_t dthres, uint8_t* out) {
+  extern __shared__ uint32_t hist[];
+  const uint2 it = items[blockIdx.x];
+  const dinq::Read R = reads[it.x];
+  const uint32_t c0 = it.y, c1 = min(c0 + P.ch, R.ntiles);
+  for (uint32_t i = threadIdx.x; i < (c1 - c0) * P.stride; i += INQ_TPB) hist[i] = 0;
+  __syncthreads();
+  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  for (uint64_t o = R.o0 + warp; o < R.o1; o += INQ_TPB / 32) dinq::add_overlap(ov[o], trace, R.alen, tspace, c0, c1, hist, P, lane, 32);
+  __syncthreads();
+  for (uint32_t t = c0 + threadIdx.x; t < c1; t += INQ_TPB)
+    out[R.out + t] = dinq::tile_byte(hist + (t - c0) * P.stride, P, dthres, tspace, ov + R.o0, R.o1 - R.o0, trace, R.alen, t);
+}
+
 // ---- pile vote (vote_core.cuh): per window the offset table, per A position the column votes (count pass, then fill pass)
 __global__ void vote_k0(const dvote::Res* res, const uint8_t* ops, uint64_t nwin, dvote::Params P, uint16_t* ent, int* err) {
   uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -574,6 +595,9 @@ struct dcu_ctx {
   DevBuf<uint8_t> dprof_scratch; DevBuf<dcu_profile_window> dprof_out;
   std::vector<dcu_profile_window> prof; uint64_t prof_host = 0;
   std::vector<uint8_t> hpacked; const uint8_t* hpacked_src = nullptr;
+  // intrinsic quality track (dcu_inqual): the batch's overlaps, trace, reads, blocks and bytes; kernel time and histogram shape of the last call
+  DevBuf<dinq::Ovl> dqovl; DevBuf<uint16_t> dqtrace; DevBuf<dinq::Read> dqreads; DevBuf<uint2> dqitems; DevBuf<uint8_t> dqout;
+  float inq_ms = 0.f; uint32_t inq_nb = 0, inq_ch = 0;
   std::string err;
 };
 
@@ -661,6 +685,7 @@ void dcu_destroy(dcu_ctx* ctx) {
   ctx->dpboff.release(); ctx->dptrace.release(); ctx->dpmin.release(); ctx->dpdiv.release(); ctx->dpact.release(); ctx->dpcnt.release(); ctx->dpblkw.release(); ctx->dpblks.release();
   ctx->dovf[0].release(); ctx->dovf[1].release(); ctx->dovf[2].release(); ctx->dcnt.release(); ctx->dslab[0].release(); ctx->dslab[1].release(); ctx->dslab[2].release();
   ctx->dprof_scratch.release(); ctx->dprof_out.release(); ctx->dslabH.release(); ctx->dovfH.release(); ctx->dvent.release(); ctx->dvflag.release(); ctx->dvblk.release(); ctx->dvchars.release(); ctx->dvreads.release(); ctx->dvbound.release();
+  ctx->dqovl.release(); ctx->dqtrace.release(); ctx->dqreads.release(); ctx->dqitems.release(); ctx->dqout.release();
   if (ctx->hwin) cudaFreeHost(ctx->hwin);
   if (ctx->ev0) cudaEventDestroy(ctx->ev0);
   if (ctx->ev1) cudaEventDestroy(ctx->ev1);
@@ -968,6 +993,51 @@ int dcu_get_profile(dcu_ctx* ctx, dcu_profile_window* rec) {
 int dcu_last_profile_stats(dcu_ctx* ctx, uint64_t* host_windows) {
   if (!ctx) return DCU_ERR_PARAM;
   if (host_windows) *host_windows = ctx->prof_host;
+  return DCU_OK;
+}
+
+// intrinsic quality track of reads [first_read, last_read): the reads' layout and the histogram shape on the host (dinq::prepare, dinq::plan),
+// one block per (read, chunk of tiles) on the device (inq_k), the bytes copied back into out_bytes.  The resident batch is not touched.
+int dcu_inqual(dcu_ctx* ctx, const dcu_overlap* ovl, uint64_t novl, const uint16_t* trace, uint64_t ntrace, int32_t tspace, const uint32_t* read_len,
+               uint64_t first_read, uint64_t last_read, uint64_t depth, uint8_t* out_bytes, uint64_t* nbytes) {
+  if (!ctx || (!ovl && novl) || (!trace && ntrace) || (!read_len && last_read > first_read) || !nbytes) return DCU_ERR_PARAM;
+  if (depth < 4) { ctx->err = "depth must be at least 4 (d / 4 contributions per tile)"; return DCU_ERR_PARAM; }
+  CK(cudaSetDevice(ctx->device));
+  const uint64_t nr = last_read > first_read ? last_read - first_read : 0;
+  std::vector<dinq::Read> R(nr);
+  uint64_t nb = 0; uint32_t maxdiff = 0;
+  const dinq::Ovl* ov = reinterpret_cast<const dinq::Ovl*>(ovl);
+  if (const char* e = dinq::prepare(ov, novl, ntrace, trace, tspace, read_len, first_read, last_read, R.data(), nb, maxdiff)) { ctx->err = e; return DCU_ERR_PARAM; }
+  if (nb && !out_bytes) return DCU_ERR_PARAM;
+  *nbytes = nb;
+  const dinq::Plan P = dinq::plan(maxdiff);
+  std::vector<uint2> items;
+  for (uint64_t r = 0; r < nr; ++r)
+    for (uint32_t c = 0; c < R[r].ntiles; c += P.ch) items.push_back(make_uint2((uint32_t)r, c));
+  if (nr >= 0xFFFFFFFFull || items.size() >= 0x7FFFFFFFull) { ctx->err = "batch too large"; return DCU_ERR_UNSUPPORTED; }
+  ctx->inq_ms = 0.f; ctx->inq_nb = P.nb; ctx->inq_ch = P.ch;
+  if (items.empty()) return DCU_OK;
+  cudaStream_t st = ctx->stream;
+  CK(ctx->dqovl.ensure(novl + 1)); CK(ctx->dqtrace.ensure(ntrace + 1)); CK(ctx->dqreads.ensure(nr)); CK(ctx->dqitems.ensure(items.size())); CK(ctx->dqout.ensure(nb));
+  if (novl) CK(cudaMemcpyAsync(ctx->dqovl.p, ov, novl * sizeof(dinq::Ovl), cudaMemcpyHostToDevice, st));
+  if (ntrace) CK(cudaMemcpyAsync(ctx->dqtrace.p, trace, ntrace * 2, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(ctx->dqreads.p, R.data(), nr * sizeof(dinq::Read), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(ctx->dqitems.p, items.data(), items.size() * sizeof(uint2), cudaMemcpyHostToDevice, st));
+  const size_t smem = (size_t)P.ch * P.stride * sizeof(uint32_t);
+  CK(cudaEventRecord(ctx->ev0, st));
+  inq_k<<<(unsigned)items.size(), INQ_TPB, smem, st>>>(ctx->dqovl.p, ctx->dqtrace.p, ctx->dqreads.p, ctx->dqitems.p, tspace, P, depth / 4, ctx->dqout.p);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(ctx->ev1, st));
+  CK(cudaMemcpyAsync(out_bytes, ctx->dqout.p, nb, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  CK(cudaEventElapsedTime(&ctx->inq_ms, ctx->ev0, ctx->ev1));
+  return DCU_OK;
+}
+int dcu_last_inqual_stats(dcu_ctx* ctx, float* kernel_ms, uint32_t* bins, uint32_t* tiles_per_block) {
+  if (!ctx) return DCU_ERR_PARAM;
+  if (kernel_ms) *kernel_ms = ctx->inq_ms;
+  if (bins) *bins = ctx->inq_nb;
+  if (tiles_per_block) *tiles_per_block = ctx->inq_ch;
   return DCU_OK;
 }
 

@@ -28,6 +28,7 @@
 #include "pile.hpp"
 #include "vote.hpp"
 #include "eprof.hpp"
+#include "args.hpp"
 #include "../../../include/daccord_b200.h"
 
 using namespace dhost;
@@ -45,26 +46,7 @@ static const char* HELP =
     "\t--vard: alignments considered per read proportional to its length, max(2v, 2v*length/average length) (default 0 = off, -D applies)\n\t-k: kmer size lo[,hi] (default 8)\n"
     "\t--device: CUDA device ordinal (default 0)\n\t--batchreads: A-reads per GPU batch (default 1024)\n\t--inflight: batches in flight on the GPU (default 3)\n";
 
-struct Args { std::map<std::string, std::string> opt; std::vector<std::string> pos; };
-static bool parse_args(int argc, char** argv, Args& A) {
-  static const char* longs[] = {"minfilterfreq", "maxfilterfreq", "vard", "eprofonly", "deepprofileonly", "keepeprof", "device", "batchreads", "inflight", "help", "version", nullptr};
-  int i = 1;
-  for (; i < argc; ++i) {
-    std::string s = argv[i];
-    if (s.size() >= 2 && s[0] == '-' && s[1] == '-') {
-      std::string body = s.substr(2), key, val; bool found = false;
-      for (int j = 0; longs[j]; ++j) { size_t n = strlen(longs[j]); if (body.compare(0, n, longs[j]) == 0 && n > key.size()) { key = longs[j]; found = true; } }
-      if (!found) { fprintf(stderr, "[E] unknown option %s\n", s.c_str()); return false; }
-      val = body.substr(key.size());
-      if (!val.empty() && val[0] == '=') val = val.substr(1);
-      A.opt[key] = val;
-    } else if (s.size() >= 2 && s[0] == '-' && !isdigit((unsigned char)s[1])) {
-      A.opt[std::string(1, s[1])] = s.substr(2);          // libmaus2 ArgParser style: value attached (-w40)
-    } else break;                                          // options must precede positionals (README.md:99)
-  }
-  for (; i < argc; ++i) A.pos.push_back(argv[i]);
-  return true;
-}
+static const char* const LONGS[] = {"minfilterfreq", "maxfilterfreq", "vard", "eprofonly", "deepprofileonly", "keepeprof", "device", "batchreads", "inflight", "help", "version", nullptr};
 static bool parse_pair(const std::string& s, int64_t& a, int64_t& b) { return sscanf(s.c_str(), "%ld,%ld", &a, &b) == 2; }
 
 static_assert(sizeof(ProfileWindow) == sizeof(dcu_profile_window) && offsetof(ProfileWindow, cnt) == offsetof(dcu_profile_window, cnt), "one record layout");
@@ -106,7 +88,7 @@ static bool gpu_profile_windows(const PackedDB& db, const LasData& las, int64_t 
 
 int main(int argc, char** argv) {
   Args A;
-  if (!parse_args(argc, argv, A)) return EXIT_FAILURE;
+  if (!parse_args(argc, argv, LONGS, A)) return EXIT_FAILURE;
   if (A.opt.count("h") || A.opt.count("help") || A.pos.size() < 2) { fprintf(stderr, "%s", HELP); return A.pos.size() < 2 && !A.opt.count("h") && !A.opt.count("help") ? EXIT_FAILURE : EXIT_SUCCESS; }
   auto getu = [&](const char* k, uint64_t def) -> uint64_t { auto it = A.opt.find(k); return (it == A.opt.end() || it->second.empty()) ? def : strtoull(it->second.c_str(), nullptr, 10); };
   // reads.las reads.db [reads2.db]: A-reads from reads.db, B-reads from reads2.db (reference src/daccord.cpp:2598-2622, :1337-1369)

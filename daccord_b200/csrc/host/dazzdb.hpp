@@ -56,7 +56,8 @@ inline void write_dazzdb(const std::string& dbfn, const PackedDB& db) {
 // them with -a), in file order (Trim_DB of the public DAZZ_DB sources).  DALIGNER numbers reads in the trimmed view, so that is the
 // numbering a .las refers to.
 enum { DAZZ_DB_BEST = 0x0400 };
-inline void read_dazzdb(const std::string& dbfn, PackedDB& db) {
+// the trimmed view's byte offsets and lengths from the .idx, every read checked against `sz`, the size of the .bps
+inline void read_dazzdb_index(const std::string& dbfn, long sz, PackedDB& db) {
   FILE* f = fopen(hidden(dbfn, ".idx").c_str(), "rb");
   if (!f) throw std::runtime_error("cannot open " + hidden(dbfn, ".idx"));
   DazzHeader h;
@@ -64,12 +65,6 @@ inline void read_dazzdb(const std::string& dbfn, PackedDB& db) {
   if (h.ureads < 0 || h.treads < 0 || h.treads > h.ureads) { fclose(f); throw std::runtime_error("implausible read counts in .idx header (not a 64-bit DAZZ_DB index?)"); }
   std::vector<DazzRead> all((size_t)h.ureads);
   if (h.ureads && fread(all.data(), sizeof(DazzRead), (size_t)h.ureads, f) != (size_t)h.ureads) { fclose(f); throw std::runtime_error("short .idx"); }
-  fclose(f);
-  f = fopen(hidden(dbfn, ".bps").c_str(), "rb");
-  if (!f) throw std::runtime_error("cannot open " + hidden(dbfn, ".bps"));
-  fseek(f, 0, SEEK_END); long sz = ftell(f); fseek(f, 0, SEEK_SET);
-  db.bytes.assign((size_t)sz + 16, 0);
-  if (sz && fread(db.bytes.data(), 1, (size_t)sz, f) != (size_t)sz) { fclose(f); throw std::runtime_error("short .bps"); }
   fclose(f);
   // trimmed view (equal to the untrimmed one when the DB was never split or was split with -x0 -a)
   db.boff.clear(); db.rlen.clear();
@@ -83,6 +78,43 @@ inline void read_dazzdb(const std::string& dbfn, PackedDB& db) {
   }
   if (trim && (int64_t)db.rlen.size() != (int64_t)h.treads)
     throw std::runtime_error("trimmed view holds " + std::to_string(db.rlen.size()) + " reads, header says " + std::to_string(h.treads) + " (cutoff / best flags not understood)");
+}
+inline void read_dazzdb(const std::string& dbfn, PackedDB& db) {
+  FILE* f = fopen(hidden(dbfn, ".bps").c_str(), "rb");
+  if (!f) throw std::runtime_error("cannot open " + hidden(dbfn, ".bps"));
+  fseek(f, 0, SEEK_END); long sz = ftell(f); fseek(f, 0, SEEK_SET);
+  db.bytes.assign((size_t)sz + 16, 0);
+  if (sz && fread(db.bytes.data(), 1, (size_t)sz, f) != (size_t)sz) { fclose(f); throw std::runtime_error("short .bps"); }
+  fclose(f);
+  read_dazzdb_index(dbfn, sz, db);
+}
+// the trimmed view without the bases (db.bytes stays empty): what a tool that needs only the read lengths loads
+inline void read_dazzdb_lengths(const std::string& dbfn, PackedDB& db) {
+  FILE* f = fopen(hidden(dbfn, ".bps").c_str(), "rb");
+  if (!f) throw std::runtime_error("cannot open " + hidden(dbfn, ".bps"));
+  fseek(f, 0, SEEK_END); const long sz = ftell(f);
+  fclose(f);
+  db.bytes.clear();
+  read_dazzdb_index(dbfn, sz, db);
+}
+// reads [first, last) of block b of a DB in its trimmed view: the whole DB for b = 0, else the b-th interval of the (ufirst, tfirst) boundary
+// lines of the .db stub that follow "blocks = n" and the "size = ..." line (DAZZ_DB's DBsplit layout)
+inline void dazzdb_block(const std::string& dbfn, int64_t b, uint64_t nreads, uint64_t& first, uint64_t& last) {
+  if (b == 0) { first = 0; last = nreads; return; }
+  FILE* f = fopen(dbfn.c_str(), "r");
+  if (!f) throw std::runtime_error("cannot open " + dbfn);
+  char line[4096]; int nblocks = -1; std::vector<int64_t> tfirst;
+  while (fgets(line, sizeof line, f)) {
+    if (nblocks < 0) { if (sscanf(line, " blocks = %d", &nblocks) != 1) nblocks = -1; else if (!fgets(line, sizeof line, f)) break; continue; }
+    long long u, t;
+    if ((int)tfirst.size() > nblocks || sscanf(line, " %lld %lld", &u, &t) != 2) break;
+    tfirst.push_back(t);
+  }
+  fclose(f);
+  if (nblocks < 0 || (int64_t)tfirst.size() != (int64_t)nblocks + 1) throw std::runtime_error("no block boundaries in " + dbfn + " (blocks = n line and n + 1 boundary lines)");
+  if (b < 0 || b > nblocks) throw std::runtime_error("block " + std::to_string(b) + " not in " + dbfn + " (" + std::to_string(nblocks) + " blocks)");
+  first = (uint64_t)tfirst[(size_t)b - 1]; last = (uint64_t)tfirst[(size_t)b];
+  if (tfirst[(size_t)b - 1] < 0 || first > last || last > nreads) throw std::runtime_error("block " + std::to_string(b) + " of " + dbfn + " lies outside its " + std::to_string(nreads) + " reads");
 }
 // one read space for an asymmetric run (`daccord reads.las A.db B.db`): B's reads are appended to A's as reads nA..nA+nB-1,
 // their byte offsets shifted past A's packed bytes.  The window kernel, the piler and the vote address reads only through

@@ -157,6 +157,20 @@ int dcu_profile(dcu_ctx* ctx, const dcu_overlap* ovl, uint64_t novl, const uint1
 int dcu_get_profile(dcu_ctx* ctx, dcu_profile_window* rec);
 /* windows of the last dcu_profile that were finished on the host */
 int dcu_last_profile_stats(dcu_ctx* ctx, uint64_t* host_windows);
+/* ---- intrinsic quality track on the GPU (computeintrinsicqv, reference src/computeintrinsicqv.cpp) --------------------------------
+ * The `inqual` track of A-reads [first_read, last_read): one byte per tile of tspace bases of every read, in read order.  Input: every
+ * overlap of those A-reads (no -D / -d selection), in .las order (grouped by ascending aread), in the form of dcu_pile, with their trace
+ * points; read_len[r] for every r < last_read; depth = the tool's -d (at least 4).  Trace point i of an overlap belongs to tile
+ * abpos / tspace + i and counts only when the overlap covers the tile's whole span (INTEGRATION.md §3).  A tile with at least depth / 4
+ * contributions gets min(floor(e * 255 + 0.5), 255), e = (sum of its depth / 4 smallest diffs / (depth / 4)) / tspace; any other tile 255.
+ * out_bytes holds sum over the reads of ceil(read_len / tspace) bytes, which *nbytes receives.  Any tspace; exact for every depth and
+ * diffs value.  Needs no dcu_set_reads; the call does not touch the context's resident batch.
+ * DCU_ERR_PARAM (dcu_last_error says why): depth < 4, an overlap outside [first_read, last_read) or out of order, outside its A-read, or
+ * its trace outside `trace`. */
+int dcu_inqual(dcu_ctx* ctx, const dcu_overlap* ovl, uint64_t novl, const uint16_t* trace, uint64_t ntrace, int32_t tspace, const uint32_t* read_len,
+               uint64_t first_read, uint64_t last_read, uint64_t depth, uint8_t* out_bytes, uint64_t* nbytes);
+/* the last dcu_inqual: its kernel's time (CUDA events), histogram bins and tiles per thread block */
+int dcu_last_inqual_stats(dcu_ctx* ctx, float* kernel_ms, uint32_t* bins, uint32_t* tiles_per_block);
 /* statistics of the last launch: kernels launched, windows that needed the large-workspace pass */
 int dcu_last_stats(dcu_ctx* ctx, uint64_t* launches, uint64_t* hard_windows);
 /* more statistics of the last launch: windows the first pass handed to the plain HBM passes, windows beyond every capacity
