@@ -42,6 +42,7 @@ __device__ unsigned long long g_stage_clk[CLK_N];
 #include "pile_host.hpp"
 #include "vote_host.hpp"
 #include "profile_core.cuh"           // namespace dprof: one window of the error-profile estimator (dcu_profile)
+#include "profile_load.cuh"           // prof_load: a profile window's slices decoded into its scratch
 #include "inqual_core.cuh"            // namespace dinq: the intrinsic quality track (dcu_inqual)
 #include "../../include/daccord_b200.h"
 
@@ -444,25 +445,8 @@ __global__ void pile_k3(const dpile::Win* win, const dpile::Sl* sl, uint64_t nwi
 
 // ---- error-profile windows (profile_core.cuh): one thread per window, grid-stride, each thread on its own PROF_SCRATCH bytes of HBM
 // scratch of prof_scratch_bytes (the hash table, marks and 7-mer bits start zeroed and are left zeroed by every window)
+// (prof_load, which decodes a window's slices into the scratch, is in profile_load.cuh)
 constexpr int PROF_TPB = 128, PROF_BLOCKS_PER_SM = 2;
-// decodes the slices of window w into S (false: beyond S's capacities)
-__host__ __device__ inline bool prof_load(const dpile::Win& w, const dpile::Sl* sl, const uint8_t* packed, const dprof::Scratch& S) {
-  if (w.slice_cnt > S.maxs) return false;
-  uint32_t tot = 0;
-  for (uint32_t j = 0; j < w.slice_cnt; ++j) { const uint32_t len = sl[w.slice_begin + j].len; if (len > S.maxlen) return false; tot += len; }
-  if (tot > S.maxb) return false;
-  uint32_t o = 0;
-  for (uint32_t j = 0; j < w.slice_cnt; ++j) {
-    const dpile::Sl x = sl[w.slice_begin + j]; S.soff[j] = o;
-    for (uint32_t i = 0; i < x.len; ++i) {
-      const uint32_t g = (x.flags & 1u) ? x.gpos + x.len - 1 - i : x.gpos + i;
-      const uint8_t b = (packed[g >> 2] >> (6 - 2 * (g & 3))) & 3;
-      S.bases[o++] = (x.flags & 1u) ? (uint8_t)(3 - b) : b;
-    }
-  }
-  S.soff[w.slice_cnt] = o;
-  return true;
-}
 __global__ void __launch_bounds__(PROF_TPB) prof_k(const dpile::Win* win, const dpile::Sl* sl, uint64_t nwin, const uint8_t* packed, uint8_t* scratch,
                                                   uint64_t stride, dcu_profile_window* out) {
   const uint64_t tid = (uint64_t)blockIdx.x * PROF_TPB + threadIdx.x, nth = (uint64_t)gridDim.x * PROF_TPB;
@@ -693,6 +677,10 @@ void dcu_destroy(dcu_ctx* ctx) {
   delete ctx;
 }
 
+// the host copy of the read database that dcu_profile decodes its host windows from is stale once the database changes: the same device
+// buffer may be refilled with other bases of the same length, so a new database always drops it
+static void drop_host_reads(dcu_ctx* ctx) { ctx->hpacked_src = nullptr; std::vector<uint8_t>().swap(ctx->hpacked); }
+
 int dcu_set_reads(dcu_ctx* ctx, const uint8_t* packed, uint64_t nbytes) {
   if (!ctx || !packed) return DCU_ERR_PARAM;
   if (nbytes >= (1ull << 30)) { ctx->err = "database larger than 2^32 bases"; return DCU_ERR_UNSUPPORTED; }
@@ -702,6 +690,7 @@ int dcu_set_reads(dcu_ctx* ctx, const uint8_t* packed, uint64_t nbytes) {
   CK(cudaMemsetAsync(ctx->dpacked_own.p + nbytes, 0, 64, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   ctx->dpacked = ctx->dpacked_own.p; ctx->packed_bytes = nbytes; ctx->packed_padded = (nbytes + 48) & ~(uint64_t)15;
+  drop_host_reads(ctx);
   return DCU_OK;
 }
 int dcu_set_reads_device(dcu_ctx* ctx, const void* dpacked, uint64_t nbytes) {
@@ -709,6 +698,7 @@ int dcu_set_reads_device(dcu_ctx* ctx, const void* dpacked, uint64_t nbytes) {
   if (nbytes >= (1ull << 30)) { ctx->err = "database larger than 2^32 bases"; return DCU_ERR_UNSUPPORTED; }
   ctx->dpacked = (const uint8_t*)dpacked; ctx->packed_bytes = nbytes; ctx->packed_padded = nbytes & ~(uint64_t)15;     // a caller's buffer: whole 16-byte chunks inside it only
   if (((uintptr_t)dpacked & 15) != 0) ctx->packed_padded = 0;      // unaligned buffer: no staging (direct loads)
+  drop_host_reads(ctx);
   return DCU_OK;
 }
 
@@ -716,6 +706,7 @@ int dcu_share_reads(dcu_ctx* ctx, dcu_ctx* owner) {
   if (!ctx || !owner || ctx->device != owner->device) return DCU_ERR_PARAM;
   if (!owner->dpacked) { ctx->err = "owner holds no read database"; return DCU_ERR_STATE; }
   ctx->dpacked = owner->dpacked; ctx->packed_bytes = owner->packed_bytes; ctx->packed_padded = owner->packed_padded;
+  drop_host_reads(ctx);
   return DCU_OK;
 }
 

@@ -84,7 +84,7 @@ int dcu_device_count(int* n);
  * concatenated offset tables (B's shifted by A's byte count) and length tables, and overlaps whose bread has A's read count added. */
 int dcu_set_reads(dcu_ctx* ctx, const uint8_t* packed, uint64_t nbytes);
 /* same, but the buffer is already resident in device memory on ctx's device (e.g. after an
- * ncclBroadcast of the database); the library does not take ownership */
+ * ncclBroadcast of the database); the library does not take ownership.  Call it again after changing the buffer's contents. */
 int dcu_set_reads_device(dcu_ctx* ctx, const void* dpacked, uint64_t nbytes);
 /* same database as `owner` (a dcu_ctx on the same device that got it through dcu_set_reads[_device]); owner must outlive ctx's use of it */
 int dcu_share_reads(dcu_ctx* ctx, dcu_ctx* owner);
