@@ -17,6 +17,7 @@ RESULT_DT = np.dtype([("status", "u1"), ("k", "u1"), ("ff", "i1"), ("clen", "u1"
                       ("ncand", "<u2"), ("elength", "<i4")])
 SEGMENT_DT = np.dtype([("aread", "<u4"), ("first", "<u4"), ("last", "<u4"), ("reserved", "<u4"), ("len", "<u8"), ("off", "<u8")])
 PROFILE_WINDOW_DT = np.dtype([("aread", "<u4"), ("astart", "<u4"), ("status", "<u4"), ("reserved", "<u4"), ("cnt", "<u4", (4,))])
+FRAGMENT_DT = np.dtype([("aread", "<u4"), ("from", "<u4"), ("to", "<u4"), ("reserved", "<u4"), ("off", "<u8"), ("len", "<u8")])
 PROF_SKIPPED, PROF_REPEAT, PROF_NO_CONSENSUS, PROF_OK = 0, 1, 2, 3
 CONS_STRIDE, OPS_STRIDE = 64, 128
 WIN_SKIPPED, WIN_OK, WIN_FAILED = 0, 1, 2
@@ -149,6 +150,29 @@ class Engine:
         ms, nb, ch = C.c_float(0), C.c_uint32(0), C.c_uint32(0)
         self._ck(self.lib.dcu_last_inqual_stats(self.ctx, C.byref(ms), C.byref(nb), C.byref(ch)))
         return {"kernel_ms": ms.value, "bins": nb.value, "tiles_per_block": ch.value}
+
+    def exqual(self, frag, codes, read_boff, read_len, tspace, first_read, last_read):
+        """the extrinsic quality track of reads [first_read, last_read) on the GPU (dcu_exqual): frag = daccord's consensus fragments of those
+        reads as FRAGMENT_DT (aread, from, to = min(last + 1, read length), off / len into codes), grouped by ascending aread; codes = one uint8
+        per fragment symbol (0..3 = ACGT, 4 = matches nothing); the read bases come from set_reads.  Returns one uint8 per tile of tspace
+        bases of every read, in read order"""
+        read_len = np.ascontiguousarray(read_len, np.uint32)
+        read_boff = np.ascontiguousarray(read_boff, np.uint64)
+        frag = np.ascontiguousarray(frag, FRAGMENT_DT)
+        codes = np.ascontiguousarray(codes, np.uint8)
+        nb = int(((read_len[first_read:last_read].astype(np.uint64) + tspace - 1) // tspace).sum())
+        out = np.zeros(max(nb, 1), np.uint8)
+        n = C.c_uint64(0)
+        self._ck(self.lib.dcu_exqual(self.ctx, _p(frag), C.c_uint64(len(frag)), _p(codes), C.c_uint64(len(codes)), _p(read_boff), _p(read_len), C.c_int32(tspace),
+                                     C.c_uint64(first_read), C.c_uint64(last_read), _p(out), C.byref(n)))
+        return out[:n.value]
+
+    def exqual_stats(self):
+        """the last exqual call: kernel time in ms (CUDA events), fragments rerun with twice the first band, fragments finished on the host
+        (dcu_last_exqual_stats)"""
+        ms, rt, hf = C.c_float(0), C.c_uint64(0), C.c_uint64(0)
+        self._ck(self.lib.dcu_last_exqual_stats(self.ctx, C.byref(ms), C.byref(rt), C.byref(hf)))
+        return {"kernel_ms": ms.value, "retried": rt.value, "host_fragments": hf.value}
 
     def get_windows(self, with_slices=False):
         win = np.zeros(self.nwin, WINDOW_DT)

@@ -42,7 +42,8 @@ def build(force=False, verbose=False):
     host_src = os.path.join(csrc, "host", "hostlib.cpp")  # noqa
     host_deps = [os.path.join(csrc, "host", f) for f in os.listdir(os.path.join(csrc, "host"))] + [os.path.join(ROOT, "include", "daccord_b200.h"),
                                                                                                os.path.join(csrc, "profile_core.cuh"),
-                                                                                               os.path.join(csrc, "inqual_core.cuh")]
+                                                                                               os.path.join(csrc, "inqual_core.cuh"),
+                                                                                               os.path.join(csrc, "exqual_core.cuh")]
     if force or _newer(HOST_LIB, host_deps):
         subprocess.check_call(["/usr/bin/g++", "-O3", "-g", "-std=c++17", "-march=x86-64-v2", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared",
                                "-o", HOST_LIB, host_src])
@@ -54,6 +55,10 @@ def build(force=False, verbose=False):
     if force or _newer(iqv, host_deps + [LIB]):
         subprocess.check_call(["/usr/bin/g++", "-O3", "-g", "-std=c++17", "-march=x86-64-v2", "-ffp-contract=off", "-fopenmp", "-pthread", "-o", iqv,
                                os.path.join(csrc, "host", "computeintrinsicqv.cpp"), "-L" + BUILD, "-ldaccord_b200", "-Wl,-rpath,$ORIGIN"])
+    xqv = os.path.join(BUILD, "computeextrinsicqv")
+    if force or _newer(xqv, host_deps + [LIB]):
+        subprocess.check_call(["/usr/bin/g++", "-O3", "-g", "-std=c++17", "-march=x86-64-v2", "-ffp-contract=off", "-fopenmp", "-pthread", "-o", xqv,
+                               os.path.join(csrc, "host", "computeextrinsicqv.cpp"), "-L" + BUILD, "-ldaccord_b200", "-Wl,-rpath,$ORIGIN"])
     return LIB
 
 

@@ -44,12 +44,14 @@ __device__ unsigned long long g_stage_clk[CLK_N];
 #include "profile_core.cuh"           // namespace dprof: one window of the error-profile estimator (dcu_profile)
 #include "profile_load.cuh"           // prof_load: a profile window's slices decoded into its scratch
 #include "inqual_core.cuh"            // namespace dinq: the intrinsic quality track (dcu_inqual)
+#include "exqual_core.cuh"            // namespace dxq: the extrinsic quality track (dcu_exqual)
 #include "../../include/daccord_b200.h"
 
 static_assert(sizeof(dcu::Slice) == sizeof(dcu_slice) && sizeof(dcu::Window) == sizeof(dcu_window) && sizeof(dcu::Result) == sizeof(dcu_result), "ABI structs");
 static_assert(sizeof(dvote::Win) == sizeof(dcu_window) && sizeof(dvote::Res) == sizeof(dcu_result), "ABI structs (vote)");
 static_assert(sizeof(dinq::Ovl) == sizeof(dcu_overlap) && offsetof(dinq::Ovl, tlen) == offsetof(dcu_overlap, tlen) && offsetof(dinq::Ovl, trace_off) == offsetof(dcu_overlap, trace_off),
               "ABI structs (inqual)");
+static_assert(sizeof(dxq::Frag) == sizeof(dcu_fragment) && offsetof(dxq::Frag, off) == offsetof(dcu_fragment, off), "ABI structs (exqual)");
 
 namespace {
 
@@ -480,6 +482,52 @@ __global__ void __launch_bounds__(INQ_TPB) inq_k(const dinq::Ovl* ov, const uint
     out[R.out + t] = dinq::tile_byte(hist + (t - c0) * P.stride, P, dthres, tspace, ov + R.o0, R.o1 - R.o0, trace, R.alen, t);
 }
 
+// ---- extrinsic quality track (exqual_core.cuh): persistent warps, one fragment per warp at a time, taken by ticket in the order `order`
+// (descending work).  A warp aligns its fragment in the band K = kband[f] with its row in shared memory and its C1 decisions in its slice of
+// the slab, then lane 0 walks the traceback into the fragment's tile bytes.  status[f]: ST_OK, ST_RETRY (score above K), ST_HOST (the band
+// does not fit the row or the slab slice).
+constexpr int XQ_WPB = 4;
+__global__ void __launch_bounds__(XQ_WPB * 32) xq_k(const dxq::Frag* fr, const uint32_t* order, uint32_t nord, const uint32_t* kband, const uint8_t* codes,
+                                                   const uint64_t* boff, const uint32_t* rlen, int32_t tspace, const uint8_t* packed, uint32_t rowcap,
+                                                   uint8_t* slab, uint64_t slab_bytes, const uint64_t* fout, uint8_t* scratch, uint8_t* status,
+                                                   unsigned int* ticket) {
+  extern __shared__ int32_t xq_rows[];
+  const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
+  int32_t* row = xq_rows + (size_t)w * rowcap;
+  uint8_t* dirs = slab + ((uint64_t)blockIdx.x * XQ_WPB + w) * slab_bytes;
+  for (;;) {
+    __syncwarp();
+    uint32_t k = 0;
+    if (lane == 0) k = atomicAdd(ticket, 1u);
+    k = __shfl_sync(0xFFFFFFFFu, k, 0);
+    if (k >= nord) break;
+    const uint32_t fi = order[k];
+    const dxq::Frag f = fr[fi];
+    const uint32_t m = f.to - f.from, n = (uint32_t)f.len, K = kband[fi];
+    const dxq::Band B = dxq::band(m, n, K, 32);
+    if (dxq::row_cells(B, 32) > rowcap || dxq::dir_bytes(B, n, 32) > slab_bytes) { if (lane == 0) status[fi] = dxq::ST_HOST; continue; }
+    const uint64_t gpos = 4 * boff[f.aread] + f.from;
+    const int32_t sc = dxq::forward(packed, gpos, m, codes + f.off, n, B, row, dirs, lane);
+    if (sc > (int32_t)K) { if (lane == 0) status[fi] = dxq::ST_RETRY; continue; }
+    if (lane == 0) {
+      dxq::traceback_tiles(packed, gpos, f, codes + f.off, rlen[f.aread], tspace, B, dirs, 32, scratch + fout[fi]);
+      status[fi] = dxq::ST_OK;
+    }
+  }
+}
+// the track of a batch: per read (one block), per tile the minimum over the read's fragments that cover it (255 where none)
+__global__ void xq_min_k(const dxq::Read* reads, const dxq::Frag* fr, const uint64_t* fout, const uint8_t* scratch, int32_t tspace, uint8_t* out) {
+  const dxq::Read R = reads[blockIdx.x];
+  for (uint32_t t = threadIdx.x; t < R.ntiles; t += blockDim.x) {
+    uint32_t v = 255;
+    for (uint64_t k = R.f0; k < R.f1; ++k) {
+      const uint32_t t0 = dxq::frag_t0(fr[k], tspace);
+      if (t >= t0 && t < t0 + dxq::frag_ntiles(fr[k], tspace)) { const uint32_t b = scratch[fout[k] + t - t0]; v = b < v ? b : v; }
+    }
+    out[R.out + t] = (uint8_t)v;
+  }
+}
+
 // ---- pile vote (vote_core.cuh): per window the offset table, per A position the column votes (count pass, then fill pass)
 __global__ void vote_k0(const dvote::Res* res, const uint8_t* ops, uint64_t nwin, dvote::Params P, uint16_t* ent, int* err) {
   uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -582,6 +630,10 @@ struct dcu_ctx {
   // intrinsic quality track (dcu_inqual): the batch's overlaps, trace, reads, blocks and bytes; kernel time and histogram shape of the last call
   DevBuf<dinq::Ovl> dqovl; DevBuf<uint16_t> dqtrace; DevBuf<dinq::Read> dqreads; DevBuf<uint2> dqitems; DevBuf<uint8_t> dqout;
   float inq_ms = 0.f; uint32_t inq_nb = 0, inq_ch = 0;
+  // extrinsic quality track (dcu_exqual): fragments, symbols, read offsets and lengths, scratch and track bytes; last call's statistics
+  DevBuf<dxq::Frag> dxfrag; DevBuf<uint8_t> dxcodes, dxscratch, dxout, dxstatus; DevBuf<uint64_t> dxboff, dxfout; DevBuf<uint32_t> dxrlen, dxorder, dxkband;
+  DevBuf<dxq::Read> dxreads; DevBuf<unsigned int> dxticket;
+  float xq_ms = 0.f; uint64_t xq_retried = 0, xq_host = 0;
   std::string err;
 };
 
@@ -670,6 +722,8 @@ void dcu_destroy(dcu_ctx* ctx) {
   ctx->dovf[0].release(); ctx->dovf[1].release(); ctx->dovf[2].release(); ctx->dcnt.release(); ctx->dslab[0].release(); ctx->dslab[1].release(); ctx->dslab[2].release();
   ctx->dprof_scratch.release(); ctx->dprof_out.release(); ctx->dslabH.release(); ctx->dovfH.release(); ctx->dvent.release(); ctx->dvflag.release(); ctx->dvblk.release(); ctx->dvchars.release(); ctx->dvreads.release(); ctx->dvbound.release();
   ctx->dqovl.release(); ctx->dqtrace.release(); ctx->dqreads.release(); ctx->dqitems.release(); ctx->dqout.release();
+  ctx->dxfrag.release(); ctx->dxcodes.release(); ctx->dxscratch.release(); ctx->dxout.release(); ctx->dxstatus.release(); ctx->dxboff.release();
+  ctx->dxfout.release(); ctx->dxrlen.release(); ctx->dxorder.release(); ctx->dxkband.release(); ctx->dxreads.release(); ctx->dxticket.release();
   if (ctx->hwin) cudaFreeHost(ctx->hwin);
   if (ctx->ev0) cudaEventDestroy(ctx->ev0);
   if (ctx->ev1) cudaEventDestroy(ctx->ev1);
@@ -1029,6 +1083,144 @@ int dcu_last_inqual_stats(dcu_ctx* ctx, float* kernel_ms, uint32_t* bins, uint32
   if (kernel_ms) *kernel_ms = ctx->inq_ms;
   if (bins) *bins = ctx->inq_nb;
   if (tiles_per_block) *tiles_per_block = ctx->inq_ch;
+  return DCU_OK;
+}
+
+// extrinsic quality track of reads [first_read, last_read): layout on the host (dxq::prepare); device passes with the band K0, then 2 K0 for
+// the fragments whose score exceeded it; fragments beyond the row or slab capacities, or above 2 K0, on the host (dxq::host_fragment on a host
+// copy of the read database); then per read the minimum over its fragments on the device.
+namespace {
+constexpr uint32_t XQ_ROWCAP_MAX = 14080 + 1;                   // int32 cells of a warp's row: 4 warps' rows in 220 KB of shared memory
+constexpr uint64_t XQ_SLAB_MAX = 256ull << 20;                  // direction bytes of one warp's fragment
+constexpr uint64_t XQ_BUDGET = 8ull << 30;                      // direction slab of one launch, at most (and at most half the free memory)
+}
+int dcu_exqual(dcu_ctx* ctx, const dcu_fragment* frag, uint64_t nfrag, const uint8_t* frag_codes, uint64_t ncodes, const uint64_t* read_boff,
+               const uint32_t* read_len, int32_t tspace, uint64_t first_read, uint64_t last_read, uint8_t* out_bytes, uint64_t* nbytes) {
+  if (!ctx || (!frag && nfrag) || (!frag_codes && ncodes) || ((!read_len || !read_boff) && last_read > first_read) || !nbytes) return DCU_ERR_PARAM;
+  if (!ctx->dpacked) { ctx->err = "dcu_set_reads not called"; return DCU_ERR_STATE; }
+  CK(cudaSetDevice(ctx->device));
+  const uint64_t nr = last_read > first_read ? last_read - first_read : 0;
+  const dxq::Frag* fr = reinterpret_cast<const dxq::Frag*>(frag);
+  std::vector<dxq::Read> R(nr); std::vector<uint64_t> fout(nfrag);
+  uint64_t nb = 0, nscr = 0;
+  if (const char* e = dxq::prepare(fr, nfrag, frag_codes, ncodes, tspace, read_len, first_read, last_read, R.data(), fout.data(), nb, nscr)) { ctx->err = e; return DCU_ERR_PARAM; }
+  for (uint64_t k = 0; k < nfrag; ++k)
+    if ((read_boff[fr[k].aread] * 4 + fr[k].to + 3) / 4 > ctx->packed_bytes) { ctx->err = "a fragment's read lies outside the read database"; return DCU_ERR_PARAM; }
+  if (nb && !out_bytes) return DCU_ERR_PARAM;
+  if (nfrag >= 0xFFFFFFFFull) { ctx->err = "batch too large"; return DCU_ERR_UNSUPPORTED; }
+  *nbytes = nb;
+  ctx->xq_ms = 0.f; ctx->xq_retried = 0; ctx->xq_host = 0;
+  if (!nr) return DCU_OK;
+  cudaStream_t st = ctx->stream;
+  CK(ctx->dxfrag.ensure(nfrag + 1)); CK(ctx->dxcodes.ensure(ncodes + 1)); CK(ctx->dxboff.ensure(last_read + 1)); CK(ctx->dxrlen.ensure(last_read + 1));
+  CK(ctx->dxfout.ensure(nfrag + 1)); CK(ctx->dxscratch.ensure(nscr + 1)); CK(ctx->dxstatus.ensure(nfrag + 1)); CK(ctx->dxorder.ensure(nfrag + 1));
+  CK(ctx->dxkband.ensure(nfrag + 1)); CK(ctx->dxreads.ensure(nr)); CK(ctx->dxout.ensure(nb + 1)); CK(ctx->dxticket.ensure(1));
+  if (nfrag) CK(cudaMemcpyAsync(ctx->dxfrag.p, fr, nfrag * sizeof(dxq::Frag), cudaMemcpyHostToDevice, st));
+  if (ncodes) CK(cudaMemcpyAsync(ctx->dxcodes.p, frag_codes, ncodes, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(ctx->dxboff.p, read_boff, last_read * 8, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(ctx->dxrlen.p, read_len, last_read * 4, cudaMemcpyHostToDevice, st));
+  if (nfrag) CK(cudaMemcpyAsync(ctx->dxfout.p, fout.data(), nfrag * 8, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(ctx->dxreads.p, R.data(), nr * sizeof(dxq::Read), cudaMemcpyHostToDevice, st));
+  // work order (descending band cells) and first band of every fragment
+  std::vector<uint32_t> K0(nfrag), kb(nfrag), list(nfrag);
+  std::vector<uint64_t> need(nfrag);
+  for (uint64_t k = 0; k < nfrag; ++k) { K0[k] = dxq::first_k(fr[k].to - fr[k].from, (uint32_t)fr[k].len); list[k] = (uint32_t)k; }
+  std::vector<uint8_t> status(nfrag, dxq::ST_HOST);
+  int occ = 0;
+  float ms_total = 0.f;
+  for (int pass = 0; pass < 2 && !list.empty(); ++pass) {
+    for (uint32_t k : list) {
+      kb[k] = K0[k] << pass;
+      const dxq::Band B = dxq::band(fr[k].to - fr[k].from, (uint32_t)fr[k].len, kb[k], 32);
+      need[k] = dxq::row_cells(B, 32) <= XQ_ROWCAP_MAX ? dxq::dir_bytes(B, (uint32_t)fr[k].len, 32) : UINT64_MAX;
+    }
+    std::stable_sort(list.begin(), list.end(), [&](uint32_t a, uint32_t b) { return need[a] > need[b]; });
+    // what fits the capacities runs on the device; the rest keeps ST_HOST
+    std::vector<uint32_t> dev;
+    for (uint32_t k : list) if (need[k] <= XQ_SLAB_MAX) dev.push_back(k); else status[k] = dxq::ST_HOST;
+    if (!dev.empty()) {
+      CK(cudaMemcpyAsync(ctx->dxorder.p, dev.data(), dev.size() * 4, cudaMemcpyHostToDevice, st));
+      CK(cudaMemcpyAsync(ctx->dxkband.p, kb.data(), nfrag * 4, cudaMemcpyHostToDevice, st));
+      size_t fmem = 0, tmem = 0;
+      CK(cudaMemGetInfo(&fmem, &tmem));
+      const uint64_t budget = std::min<uint64_t>(XQ_BUDGET, fmem / 2);
+      // launches over runs of similar size: a run starts at the largest remaining fragment and takes every fragment needing at least half of it
+      uint64_t r0 = 0;
+      uint8_t* slab = nullptr;
+      while (r0 < dev.size()) {
+        const uint64_t top = std::max<uint64_t>(need[dev[r0]], 1);
+        uint64_t r1 = r0 + 1;
+        while (r1 < dev.size() && need[dev[r1]] * 2 >= top) ++r1;
+        uint32_t rowcap = 0;
+        for (uint64_t q = r0; q < r1; ++q) {
+          const dxq::Frag& f = fr[dev[q]];
+          rowcap = std::max<uint32_t>(rowcap, (uint32_t)dxq::row_cells(dxq::band(f.to - f.from, (uint32_t)f.len, kb[dev[q]], 32), 32));
+        }
+        const size_t smem = (size_t)XQ_WPB * rowcap * 4;
+        CK(cudaFuncSetAttribute(xq_k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, xq_k, XQ_WPB * 32, smem));
+        uint64_t blocks = std::min<uint64_t>((uint64_t)std::max(occ, 1) * ctx->num_sms, (r1 - r0 + XQ_WPB - 1) / XQ_WPB);
+        blocks = std::min<uint64_t>(blocks, std::max<uint64_t>(budget / (top * XQ_WPB), 1));
+        CK(cudaMalloc((void**)&slab, blocks * XQ_WPB * top));
+        CK(cudaMemsetAsync(ctx->dxticket.p, 0, 4, st));
+        CK(cudaEventRecord(ctx->ev0, st));
+        xq_k<<<(unsigned)blocks, XQ_WPB * 32, smem, st>>>(ctx->dxfrag.p, ctx->dxorder.p + r0, (uint32_t)(r1 - r0), ctx->dxkband.p, ctx->dxcodes.p, ctx->dxboff.p,
+                                                          ctx->dxrlen.p, tspace, ctx->dpacked, rowcap, slab, top, ctx->dxfout.p, ctx->dxscratch.p,
+                                                          ctx->dxstatus.p, ctx->dxticket.p);
+        const cudaError_t le = cudaGetLastError();
+        CK(cudaEventRecord(ctx->ev1, st));
+        const cudaError_t se = cudaStreamSynchronize(st);
+        cudaFree(slab); slab = nullptr;
+        CK(le); CK(se);
+        float ms = 0.f; CK(cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1)); ms_total += ms;
+        r0 = r1;
+      }
+      std::vector<uint8_t> sd(nfrag);
+      CK(cudaMemcpy(sd.data(), ctx->dxstatus.p, nfrag, cudaMemcpyDeviceToHost));
+      for (uint32_t k : dev) status[k] = sd[k];
+    }
+    std::vector<uint32_t> next;
+    for (uint32_t k : list) if (status[k] == dxq::ST_RETRY) next.push_back(k);
+    if (pass == 0) ctx->xq_retried = next.size();
+    list.swap(next);
+  }
+  // the host: fragments beyond the capacities, or above twice the first band
+  std::vector<uint32_t> host;
+  for (uint64_t k = 0; k < nfrag; ++k) if (status[k] != dxq::ST_OK) host.push_back((uint32_t)k);
+  if (!host.empty()) {
+    if (ctx->hpacked_src != ctx->dpacked || ctx->hpacked.size() != ctx->packed_bytes) {
+      ctx->hpacked.resize(ctx->packed_bytes);
+      CK(cudaMemcpy(ctx->hpacked.data(), ctx->dpacked, ctx->packed_bytes, cudaMemcpyDeviceToHost));
+      ctx->hpacked_src = ctx->dpacked;
+    }
+    std::vector<std::vector<uint8_t>> hb(host.size());
+#pragma omp parallel for schedule(dynamic, 1)
+    for (int64_t q = 0; q < (int64_t)host.size(); ++q) {
+      const dxq::Frag& f = fr[host[q]];
+      std::vector<uint8_t> dirs; std::vector<int32_t> row;
+      hb[q].resize(dxq::frag_ntiles(f, tspace));
+      const uint32_t K = dxq::first_k(f.to - f.from, (uint32_t)f.len) * (status[host[q]] == dxq::ST_RETRY ? 4u : 1u);
+      dxq::host_fragment(ctx->hpacked.data(), read_boff[f.aread], f, frag_codes, read_len[f.aread], tspace, K, dirs, row, hb[q].data(), nullptr);
+    }
+    for (size_t q = 0; q < host.size(); ++q) CK(cudaMemcpyAsync(ctx->dxscratch.p + fout[host[q]], hb[q].data(), hb[q].size(), cudaMemcpyHostToDevice, st));
+    CK(cudaStreamSynchronize(st));
+    ctx->xq_host = host.size();
+  }
+  CK(cudaEventRecord(ctx->ev0, st));
+  xq_min_k<<<(unsigned)nr, 128, 0, st>>>(ctx->dxreads.p, ctx->dxfrag.p, ctx->dxfout.p, ctx->dxscratch.p, tspace, ctx->dxout.p);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(ctx->ev1, st));
+  if (nb) CK(cudaMemcpyAsync(out_bytes, ctx->dxout.p, nb, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  float ms = 0.f; CK(cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1));
+  ctx->xq_ms = ms_total + ms;
+  return DCU_OK;
+}
+int dcu_last_exqual_stats(dcu_ctx* ctx, float* kernel_ms, uint64_t* retried, uint64_t* host_fragments) {
+  if (!ctx) return DCU_ERR_PARAM;
+  if (kernel_ms) *kernel_ms = ctx->xq_ms;
+  if (retried) *retried = ctx->xq_retried;
+  if (host_fragments) *host_fragments = ctx->xq_host;
   return DCU_OK;
 }
 

@@ -171,6 +171,24 @@ int dcu_inqual(dcu_ctx* ctx, const dcu_overlap* ovl, uint64_t novl, const uint16
                uint64_t first_read, uint64_t last_read, uint64_t depth, uint8_t* out_bytes, uint64_t* nbytes);
 /* the last dcu_inqual: its kernel's time (CUDA events), histogram bins and tiles per thread block */
 int dcu_last_inqual_stats(dcu_ctx* ctx, float* kernel_ms, uint32_t* bins, uint32_t* tiles_per_block);
+/* ---- extrinsic quality track on the GPU (computeextrinsicqv, reference src/computeextrinsicqv.cpp) ------------------------------
+ * The `exqual` track of reads [first_read, last_read): one byte per tile of tspace bases of every read, in read order (out_bytes holds the
+ * sum over the reads of ceil(read_len / tspace) bytes, which *nbytes receives).  Input: daccord's consensus fragments of those reads, grouped
+ * by ascending aread; fragment k aligns read aread's bases [from, to) (the header's A=[first,last]: from = first, to = min(last + 1, read
+ * length)) against frag_codes[off, off + len), one byte per symbol: 0..3 for A C G T, 4 for a symbol that matches nothing.  read_boff /
+ * read_len: byte offset and length of every read r < last_read in the database of dcu_set_reads, which holds the bases.  Per fragment, a
+ * unit-cost global alignment with traceback rule C1 (INTEGRATION.md section 3c); a tile the fragment covers whole (or the read's short last
+ * tile, when the fragment reaches the read's end) gets floor(e * 255 + 0.5), e = (mismatches + insertions + deletions) / steps of the
+ * alignment steps on the tile; the track keeps the minimum over the read's fragments and 255 where none covers a tile.  The resident
+ * batch is not touched.
+ * DCU_ERR_PARAM (dcu_last_error says why): tspace < 1, a fragment outside [first_read, last_read), out of order, with from >= to or to beyond
+ * its read, its symbols outside frag_codes or a code above 4; DCU_ERR_STATE without dcu_set_reads. */
+typedef struct dcu_fragment { uint32_t aread, from, to, reserved; uint64_t off, len; } dcu_fragment;
+int dcu_exqual(dcu_ctx* ctx, const dcu_fragment* frag, uint64_t nfrag, const uint8_t* frag_codes, uint64_t ncodes, const uint64_t* read_boff,
+               const uint32_t* read_len, int32_t tspace, uint64_t first_read, uint64_t last_read, uint8_t* out_bytes, uint64_t* nbytes);
+/* the last dcu_exqual: its kernels' time (CUDA events), fragments rerun with twice the first band, fragments finished on the host (their band
+ * did not fit the device capacities, or their score exceeded twice the first band) */
+int dcu_last_exqual_stats(dcu_ctx* ctx, float* kernel_ms, uint64_t* retried, uint64_t* host_fragments);
 /* statistics of the last launch: kernels launched, windows that needed the large-workspace pass */
 int dcu_last_stats(dcu_ctx* ctx, uint64_t* launches, uint64_t* hard_windows);
 /* more statistics of the last launch: windows the first pass handed to the plain HBM passes, windows beyond every capacity
