@@ -196,12 +196,23 @@ class Engine:
         self._ck(self.lib.dcu_run(self.ctx, _p(win), C.c_uint64(len(win)), _p(sl), C.c_uint64(len(sl)), _p(res), _p(cons), _p(ops)))
         return res, cons, ops
 
-    def vote(self, producefull=False, minlen=0, read_boff=None, read_len=None, chars_out=None):
+    def set_results(self, res, cons, ops):
+        """results of the resident batch from the caller instead of launch (dcu_set_results): RESULT_DT records and the consensus /
+        placement arenas in the layout download returns; vote then votes them"""
+        res = np.ascontiguousarray(res, RESULT_DT)
+        cons, ops = np.ascontiguousarray(cons, np.uint8), np.ascontiguousarray(ops, np.uint8)
+        assert len(res) == self.nwin and len(cons) >= self.nwin * CONS_STRIDE and len(ops) >= self.nwin * OPS_STRIDE
+        self._ck(self.lib.dcu_set_results(self.ctx, _p(res), _p(cons), _p(ops)))
+
+    def vote(self, producefull=False, minlen=0, read_boff=None, read_len=None, chars_out=None, full_reads=None):
         """pile vote of the resident results on the GPU; returns (segments, chars) -- see dcu_vote in include/daccord_b200.h.
-        chars_out: optional uint8 buffer (e.g. pinned host memory) the corrected bases are copied into when it is large enough"""
+        chars_out: optional uint8 buffer (e.g. pinned host memory) the corrected bases are copied into when it is large enough;
+        full_reads (-f): the batch's A-reads with at least one selected overlap, ascending (those without windows are printed in lower case)"""
         ns, nc = C.c_uint64(0), C.c_uint64(0)
         nreads = 0 if read_len is None else len(read_len)
-        self._ck(self.lib.dcu_vote(self.ctx, C.c_int(1 if producefull else 0), C.c_uint64(minlen), _p(read_boff), _p(read_len), C.c_uint64(nreads), C.byref(ns), C.byref(nc)))
+        fr = None if full_reads is None else np.ascontiguousarray(full_reads, np.uint32)
+        self._ck(self.lib.dcu_vote(self.ctx, C.c_int(1 if producefull else 0), C.c_uint64(minlen), _p(read_boff), _p(read_len), C.c_uint64(nreads),
+                                   _p(fr), C.c_uint64(0 if fr is None else len(fr)), C.byref(ns), C.byref(nc)))
         seg = np.zeros(ns.value, SEGMENT_DT)
         chars = chars_out[:nc.value] if (chars_out is not None and len(chars_out) >= nc.value) else np.zeros(nc.value, np.uint8)
         self._ck(self.lib.dcu_get_corrected(self.ctx, _p(seg), _p(chars)))

@@ -620,6 +620,7 @@ struct dcu_ctx {
   // vote scratch and results
   DevBuf<uint16_t> dvent; DevBuf<uint8_t> dvflag; DevBuf<uint64_t> dvblk; DevBuf<char> dvchars; DevBuf<dvote::Read> dvreads; DevBuf<dvote::Bound> dvbound;
   std::vector<dcu_segment> segs; uint64_t nchars = 0; bool results_valid = false;
+  bool has_batch = false;                                  // a batch of dcu_upload / dcu_pile is resident (dcu_set_results)
   dcu_window* hwin = nullptr; uint64_t hwin_cap = 0;      // pinned host copy of the window descriptors (dcu_vote lays out the reads from it)
   unsigned int launch_seq = 0;
   uint64_t launches = 0, hard = 0, second = 0, lost = 0;     // second: windows the shared-memory pass handed on; hard: windows of the large-workspace pass; lost: beyond every capacity
@@ -835,7 +836,7 @@ static int finish_batch(dcu_ctx* ctx, int maxS, int maxB, uint64_t totS, uint64_
     ctx->hybrid_ok = ctx->use_hybrid && !ctx->use_smem && ctx->prm.max_ff >= 2 && mean >= mind && maxB < 32768 && BPS * per_block <= (size_t)ctx->smem_optin + 1024 && per_block <= (size_t)ctx->smem_optin;
     CK(ctx->dovfH.ensure(nwin + 1));
   }
-  ctx->nwin = nwin; ctx->nsl = nsl; ctx->results_valid = false;
+  ctx->nwin = nwin; ctx->nsl = nsl; ctx->results_valid = false; ctx->has_batch = true;
   return DCU_OK;
 }
 
@@ -978,7 +979,7 @@ int dcu_profile(dcu_ctx* ctx, const dcu_overlap* ovl, uint64_t novl, const uint1
   int rc = pile_impl(ctx, ovl, novl, trace, ntrace, tspace, read_boff, read_len, nreads, 40, 5, maxalign, true, &tw, &ts, mx);
   if (rc) return rc;
   // the piles of dcu_profile are not a resident batch of the window kernel
-  ctx->nwin = 0; ctx->nsl = 0; ctx->results_valid = false;
+  ctx->nwin = 0; ctx->nsl = 0; ctx->results_valid = false; ctx->has_batch = false;
   Laps laps("dcu_profile");
   ctx->prof.resize(tw);
   if (tw) {
@@ -1449,15 +1450,33 @@ int dcu_download(dcu_ctx* ctx, dcu_result* res, uint8_t* cons, uint8_t* ops) {
   return DCU_OK;
 }
 
+// results of the resident batch from the caller instead of dcu_launch (the same layout dcu_download returns)
+int dcu_set_results(dcu_ctx* ctx, const dcu_result* res, const uint8_t* cons, const uint8_t* ops) {
+  if (!ctx) return DCU_ERR_PARAM;
+  if (!ctx->has_batch) { ctx->err = "dcu_set_results needs a resident batch (dcu_upload or dcu_pile)"; return DCU_ERR_STATE; }
+  if (ctx->nwin && (!res || !cons || !ops)) return DCU_ERR_PARAM;
+  CK(cudaSetDevice(ctx->device));
+  if (ctx->nwin) {
+    CK(cudaMemcpyAsync(ctx->dres.p, res, ctx->nwin * sizeof(dcu_result), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->dcons.p, cons, ctx->nwin * DCU_CONS_STRIDE, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->dops.p, ops, ctx->nwin * DCU_OPS_STRIDE, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  }
+  ctx->results_valid = true;
+  return DCU_OK;
+}
+
 // pile vote of the resident batch on the device (vote_core.cuh)
-int dcu_vote(dcu_ctx* ctx, int producefull, uint64_t minlen, const uint64_t* read_boff, const uint32_t* read_len, uint64_t nreads, uint64_t* nseg, uint64_t* nchars) {
+int dcu_vote(dcu_ctx* ctx, int producefull, uint64_t minlen, const uint64_t* read_boff, const uint32_t* read_len, uint64_t nreads,
+             const uint32_t* full_reads, uint64_t nfull, uint64_t* nseg, uint64_t* nchars) {
   if (!ctx) return DCU_ERR_PARAM;
   CK(cudaSetDevice(ctx->device));
   ctx->segs.clear(); ctx->nchars = 0;
   if (nseg) *nseg = 0;
   if (nchars) *nchars = 0;
-  if (!ctx->nwin) return DCU_OK;
-  if (!ctx->results_valid) { ctx->err = "dcu_vote needs the results of dcu_launch"; return DCU_ERR_STATE; }
+  if (!producefull || !full_reads) nfull = 0;
+  if (!ctx->nwin && !nfull) return DCU_OK;                 // (under -f, reads with overlaps and no window still give a record)
+  if (ctx->nwin && !ctx->results_valid) { ctx->err = "dcu_vote needs the results of dcu_launch"; return DCU_ERR_STATE; }
   if (ctx->prm.w > 127) { ctx->err = "vote tables hold w <= 127"; return DCU_ERR_UNSUPPORTED; }
   cudaStream_t st = ctx->stream;
   const uint64_t nwin = ctx->nwin;
@@ -1469,25 +1488,25 @@ int dcu_vote(dcu_ctx* ctx, int producefull, uint64_t minlen, const uint64_t* rea
     ctx->hwin_cap = nwin + nwin / 4 + 16;
   }
   dcu_window* const hwin_p = ctx->hwin;
-  CK(cudaMemcpyAsync(hwin_p, ctx->dwin.p, nwin * sizeof(dcu_window), cudaMemcpyDeviceToHost, st));
+  if (nwin) CK(cudaMemcpyAsync(hwin_p, ctx->dwin.p, nwin * sizeof(dcu_window), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   laps.lap("windows_d2h");
   dvote::Layout L;
-  if (!dvote::layout_reads(hwin_p, nwin, ctx->prm.w, producefull != 0, read_boff, read_len, nreads, L)) { ctx->err = L.err; return DCU_ERR_PARAM; }
+  if (!dvote::layout_reads(hwin_p, nwin, ctx->prm.w, producefull != 0, read_boff, read_len, nreads, L, full_reads, nfull)) { ctx->err = L.err; return DCU_ERR_PARAM; }
   laps.lap("layout");
   if (producefull) for (auto& R : L.reads) if (R.boff + (R.rlen + 3) / 4 > ctx->packed_bytes) { ctx->err = "read outside the packed database"; return DCU_ERR_PARAM; }
   const uint32_t nr = (uint32_t)L.reads.size();
   const uint64_t npos = L.npos, nblk = (npos + VOTE_TPB - 1) / VOTE_TPB;
   if (nblk >= 0x7FFFFFFFull) { ctx->err = "batch too large for the vote"; return DCU_ERR_UNSUPPORTED; }
   const uint64_t bound_cap = 2 * (nwin + nr) + 16;
-  CK(ctx->dvent.ensure(nwin * (ctx->prm.w + 1))); CK(ctx->dvflag.ensure(npos + 1)); CK(ctx->dvblk.ensure(nblk + 2)); CK(ctx->dvreads.ensure(nr + 1));
+  CK(ctx->dvent.ensure(nwin * (ctx->prm.w + 1) + 1)); CK(ctx->dvflag.ensure(npos + 1)); CK(ctx->dvblk.ensure(nblk + 2)); CK(ctx->dvreads.ensure(nr + 1));
   CK(ctx->dvbound.ensure(bound_cap)); CK(ctx->dcnt.ensure(16));
   CK(cudaMemcpyAsync(ctx->dvreads.p, L.reads.data(), nr * sizeof(dvote::Read), cudaMemcpyHostToDevice, st));
   CK(cudaMemsetAsync(ctx->dcnt.p + 4, 0, 4 * sizeof(unsigned int), st));
   int* derr = (int*)(ctx->dcnt.p + 4); unsigned int* dnb = ctx->dcnt.p + 5;
   dvote::Params vp; vp.w = ctx->prm.w; vp.cons_stride = DCU_CONS_STRIDE; vp.ops_stride = DCU_OPS_STRIDE; vp.producefull = producefull ? 1 : 0;
   dvote::Ctx vc; vc.win = (const dvote::Win*)ctx->dwin.p; vc.res = (const dvote::Res*)ctx->dres.p; vc.cons = ctx->dcons.p; vc.ent = ctx->dvent.p; vc.packed = ctx->dpacked; vc.P = vp;
-  vote_k0<<<(unsigned)((nwin + 255) / 256), 256, 0, st>>>((const dvote::Res*)ctx->dres.p, ctx->dops.p, nwin, vp, ctx->dvent.p, derr);
+  if (nwin) vote_k0<<<(unsigned)((nwin + 255) / 256), 256, 0, st>>>((const dvote::Res*)ctx->dres.p, ctx->dops.p, nwin, vp, ctx->dvent.p, derr);
   vote_k1<<<(unsigned)nblk, VOTE_TPB, 0, st>>>(vc, ctx->dvreads.p, nr, npos, ctx->dvflag.p, ctx->dvblk.p, nullptr, nullptr, nullptr, 0u);
   vote_kscan<<<1, VOTE_TPB, 0, st>>>(ctx->dvblk.p, nblk);
   CK(cudaGetLastError());

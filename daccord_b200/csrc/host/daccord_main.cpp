@@ -258,6 +258,10 @@ int main(int argc, char** argv) {
         const int64_t b0 = minaread + bi * (int64_t)batchreads, b1 = std::min<int64_t>(b0 + (int64_t)batchreads, toparead), nr = b1 - b0;
         std::vector<dcu_window> win; std::vector<dcu_slice> sl; std::vector<uint64_t> first(nr + 1, 0);
         uint64_t nw = 0, ns = 0; int rc = 0;
+        // -f prints every read with a selected overlap, in lower case where no window could be placed (reference :2543); a read whose piling
+        // failed is skipped whole, as the reference swallows its exception
+        std::vector<uint8_t> has_ovl(nr, 0);
+        for (int64_t r = 0; r < nr; ++r) has_ovl[r] = las.aidx[b0 + r] < las.aidx[b0 + r + 1] && read_limit(db.rlen[b0 + r], maxinput, vard, avglen) > 0;
         // stage 1: windows + slices -- on the GPU from the selected overlaps (dcu_pile), or by the host piler (dcu_upload)
         if (gpu_pile) {
           std::vector<std::vector<uint32_t>> sels(nr);
@@ -280,7 +284,7 @@ int main(int argc, char** argv) {
               catch (std::exception& e) {       // per-read failures are logged and skipped (reference src/daccord.cpp:2466-2478)
 #pragma omp critical
                 { fprintf(stderr, "[E] read %ld: %s\n", (long)(b0 + i), e.what()); }
-                wv[i].clear(); sv[i].clear();
+                wv[i].clear(); sv[i].clear(); has_ovl[i] = 0;
               }
             }
           }
@@ -301,7 +305,9 @@ int main(int argc, char** argv) {
         if (gpu_vote) {
           rc = dcu_download(ctx, res.data(), nullptr, nullptr);
           uint64_t nseg = 0, nch = 0;
-          if (!rc) rc = dcu_vote(ctx, producefull ? 1 : 0, minlen, db.boff.data(), db.rlen.data(), db.rlen.size(), &nseg, &nch);
+          std::vector<uint32_t> full_reads;
+          if (producefull) for (int64_t r = 0; r < nr; ++r) if (has_ovl[r]) full_reads.push_back((uint32_t)(b0 + r));
+          if (!rc) rc = dcu_vote(ctx, producefull ? 1 : 0, minlen, db.boff.data(), db.rlen.data(), db.rlen.size(), full_reads.data(), full_reads.size(), &nseg, &nch);
           seg.resize(nseg); chars.resize(nch + 1);
           if (!rc) rc = dcu_get_corrected(ctx, seg.data(), chars.data());
           if (rc) { fail(std::string("dcu_vote: ") + dcu_strerror(rc) + ": " + dcu_last_error(ctx)); break; }
@@ -314,7 +320,7 @@ int main(int argc, char** argv) {
           parts.resize(nr);
 #pragma omp parallel for schedule(dynamic, 4) num_threads(wthreads)
           for (int64_t i = 0; i < nr; ++i) {
-            if (first[i] == first[i + 1]) continue;
+            if (first[i] == first[i + 1] && !(producefull && has_ovl[i])) continue;      // see has_ovl
             std::vector<PileElement> PV;
             for (uint64_t wi = first[i]; wi < first[i + 1]; ++wi) if (res[wi].status == DCU_WIN_OK) place_window(win[wi], res[wi], cons.data() + wi * DCU_CONS_STRIDE, ops.data() + wi * DCU_OPS_STRIDE, PV);
             std::string ab;

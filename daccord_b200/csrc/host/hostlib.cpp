@@ -32,6 +32,7 @@ struct dh_data {
 struct dh_batch {
   std::vector<dcu_window> win; std::vector<dcu_slice> sl;
   std::vector<uint64_t> read_first;     // per processed read: first window index (size nreads_in_batch+1)
+  std::vector<uint8_t> has_ovl;         // per processed read: at least one selected overlap (what -f prints, with or without windows)
   uint64_t first_read = 0, last_read = 0;
   std::string err;
 };
@@ -158,6 +159,11 @@ dh_batch* dh_pile_vard(dh_data* d, uint64_t first_read, uint64_t last_read, uint
   }
   if (!err.empty()) { fprintf(stderr, "[E] %s\n", err.c_str()); return nullptr; }
   B->read_first.assign(nr + 1, 0);
+  B->has_ovl.assign(nr, 0);
+  for (uint64_t i = 0; i < nr; ++i) {
+    const uint64_t r = first_read + i;
+    B->has_ovl[i] = d->las.aidx[r] < d->las.aidx[r + 1] && read_limit(d->db.rlen[r], maxinput, vard, avglen) > 0;
+  }
   uint64_t nw = 0, ns = 0;
   for (uint64_t i = 0; i < nr; ++i) { B->read_first[i] = nw; nw += wv[i].size(); ns += sv[i].size(); }
   B->read_first[nr] = nw;
@@ -173,6 +179,26 @@ dh_batch* dh_pile_vard(dh_data* d, uint64_t first_read, uint64_t last_read, uint
 }
 dh_batch* dh_pile(dh_data* d, uint64_t first_read, uint64_t last_read, uint32_t w, uint32_t a, uint64_t maxalign, uint64_t maxinput, int nthreads) {
   return dh_pile_vard(d, first_read, last_read, w, a, maxalign, maxinput, 0, nthreads);
+}
+// a batch of given windows over A-reads [first_read, last_read) of d, grouped by ascending aread and ordered by astart inside a read
+// (no slices: what the vote needs).  has_ovl: per read of the range, whether it has a selected overlap (null: the reads with windows)
+dh_batch* dh_batch_make(dh_data* d, uint64_t first_read, uint64_t last_read, const dcu_window* win, uint64_t nwin, const uint8_t* has_ovl) {
+  if (last_read > d->nA || first_read > last_read) { d->err = "read range outside the database"; return nullptr; }
+  std::unique_ptr<dh_batch> B(new dh_batch());
+  B->first_read = first_read; B->last_read = last_read;
+  const uint64_t nr = last_read - first_read;
+  B->win.assign(win, win + nwin);
+  B->read_first.assign(nr + 1, 0);
+  uint64_t wi = 0;
+  for (uint64_t i = 0; i < nr; ++i) {
+    B->read_first[i] = wi;
+    while (wi < nwin && win[wi].aread == first_read + i) { if (wi > B->read_first[i] && win[wi].astart < win[wi - 1].astart) break; ++wi; }
+  }
+  B->read_first[nr] = wi;
+  if (wi != nwin) { d->err = "windows must lie in the read range, grouped by ascending A-read and ordered by astart"; return nullptr; }
+  B->has_ovl.resize(nr);
+  for (uint64_t i = 0; i < nr; ++i) B->has_ovl[i] = has_ovl ? (has_ovl[i] != 0) : (B->read_first[i] < B->read_first[i + 1]);
+  return B.release();
 }
 void dh_batch_destroy(dh_batch* b) { delete b; }
 
@@ -227,10 +253,11 @@ char* dh_vote(dh_data* d, dh_batch* b, const dcu_result* res, const uint8_t* con
     std::vector<PileElement> PV;
     for (uint64_t wi = b->read_first[i]; wi < b->read_first[i + 1]; ++wi)
       if (res[wi].status == DCU_WIN_OK) place_window(b->win[wi], res[wi], cons + wi * DCU_CONS_STRIDE, ops + wi * DCU_OPS_STRIDE, PV);
-    if (b->read_first[i] == b->read_first[i + 1] && !VP.producefull) continue;
+    // a read without windows prints nothing, except under -f when it has a selected overlap: the reference then fills the whole read in
+    // lower case (:2543 tests `producefull && ita != ite`, whether or not a window was placed); a read without overlaps prints nothing
+    if (b->read_first[i] == b->read_first[i + 1] && !(VP.producefull && b->has_ovl[i])) continue;
     std::string ab;
     if (VP.producefull) { std::vector<uint8_t> codes; decode_read(d->db, (uint32_t)(b->first_read + i), false, codes); ab.resize(codes.size()); for (size_t k = 0; k < codes.size(); ++k) ab[k] = "ACGT"[codes[k]]; }
-    if (b->read_first[i] == b->read_first[i + 1]) continue;      // reads without overlaps are not visited by the reference loop body either
     uint64_t c0 = 0;
     vote_read((int64_t)(b->first_read + i), PV, VP, ab, c0, parts[i]);
     cnt[i] = c0;

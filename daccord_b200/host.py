@@ -19,7 +19,7 @@ def lib():
             raise DcuError("host library %s not built: run `python -m daccord_b200.build`" % HOST_LIB_PATH)
         L = C.CDLL(HOST_LIB_PATH)
         for f in ("dh_sim_create", "dh_sim_create_ex", "dh_sim_create_spread", "dh_data_load", "dh_data_load2", "dh_pile_vard", "dh_select_overlaps_vard", "dh_data_load_range", "dh_pile", "dh_vote", "dh_data_packed", "dh_batch_windows", "dh_batch_slices", "dh_batch_read_first",
-                  "dh_select_overlaps", "dh_select_overlaps_mode", "dh_profile_windows", "dh_ovlset_data", "dh_data_trace", "dh_data_boff", "dh_data_rlen", "dh_format_segments"):
+                  "dh_select_overlaps", "dh_select_overlaps_mode", "dh_profile_windows", "dh_ovlset_data", "dh_data_trace", "dh_data_boff", "dh_data_rlen", "dh_format_segments", "dh_batch_make"):
             getattr(L, f).restype = C.c_void_p
         for f in ("dh_data_nreads", "dh_data_nall", "dh_data_novl", "dh_data_totlen"):
             getattr(L, f).restype = C.c_uint64
@@ -192,6 +192,19 @@ class Batch:
         self.sl = np.frombuffer((C.c_uint8 * (n.value * 8)).from_address(p), dtype=SLICE_DT) if n.value else np.zeros(0, SLICE_DT)
         p = lib().dh_batch_read_first(self.h, C.byref(n))
         self.read_first = np.frombuffer((C.c_uint8 * (n.value * 8)).from_address(p), dtype=np.uint64)
+
+    @staticmethod
+    def from_windows(ds, win, first, last, has_ovl=None):
+        """a batch of the given windows (WINDOW_DT, grouped by ascending aread in [first, last), ordered by astart) over the reads of ds, without
+        slices: for voting crafted results.  has_ovl: per read of [first, last), whether it has a selected overlap (default: it has windows)"""
+        win = np.ascontiguousarray(win, WINDOW_DT)
+        ho = None if has_ovl is None else np.ascontiguousarray(has_ovl, np.uint8)
+        assert ho is None or len(ho) == last - first
+        h = lib().dh_batch_make(ds.h, C.c_uint64(first), C.c_uint64(last), win.ctypes.data_as(C.c_void_p), C.c_uint64(len(win)),
+                                None if ho is None else ho.ctypes.data_as(C.c_void_p))
+        if not h:
+            raise DcuError(lib().dh_data_error(ds.h).decode())
+        return Batch(ds, h)
 
     def vote(self, res, cons, ops, producefull=False, minlen=0, counter=0, nthreads=0):
         """pile vote + FastA text (bytes) for the reads of this batch; returns (fasta, next counter)"""

@@ -132,8 +132,17 @@ int dcu_get_windows(dcu_ctx* ctx, dcu_window* win, dcu_slice* sl /* may be NULL 
  * A segment is one output sequence of the reference (:2710-2724): its FastA header is
  * ">{aread+1}/{counter}/{first}_{first+len} A=[{first},{last}]", its bases chars[off .. off+len). */
 typedef struct dcu_segment { uint32_t aread, first, last, reserved; uint64_t len, off; } dcu_segment;
+/* full_reads / nfull (producefull only, may be NULL / 0): the A-reads of the batch with at least one selected overlap, ascending.
+ * Under -f the reference prints such a read in lower case even when no window of it could be placed (:2543); a listed read
+ * without windows therefore gives one segment [0, rlen - 1] of its uncorrected bases when rlen - 1 >= 100.  Reads that are not
+ * listed and have no window give nothing. */
 int dcu_vote(dcu_ctx* ctx, int producefull, uint64_t minlen, const uint64_t* read_boff, const uint32_t* read_len, uint64_t nreads,
-             uint64_t* nseg, uint64_t* nchars);
+             const uint32_t* full_reads, uint64_t nfull, uint64_t* nseg, uint64_t* nchars);
+/* results of the resident batch (after dcu_upload or dcu_pile) given by the caller instead of computed by dcu_launch: nwin records,
+ * nwin * DCU_CONS_STRIDE consensus bytes and nwin * DCU_OPS_STRIDE placement steps, the layout of dcu_download.  dcu_vote then votes
+ * them; a placement trace that does not cover exactly w A bases makes dcu_vote fail with DCU_ERR_STATE.  DCU_ERR_STATE without a
+ * resident batch. */
+int dcu_set_results(dcu_ctx* ctx, const dcu_result* res, const uint8_t* cons, const uint8_t* ops);
 /* segments (in A-read, position order) and the character buffer (nchars bytes) of the last dcu_vote */
 int dcu_get_corrected(dcu_ctx* ctx, dcu_segment* seg, char* chars);
 /* ---- error-profile windows on the GPU -------------------------------------------------------------------------------
