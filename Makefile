@@ -9,9 +9,9 @@ CSRC     := daccord_b200/csrc
 NVFLAGS  := -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -fmad=false -Xcompiler -fPIC,-O3,-ffp-contract=off,-fopenmp -shared
 CXXFLAGS := -O3 -g -std=c++17 -march=x86-64-v2 -ffp-contract=off -fopenmp -pthread
 CUDEPS   := $(wildcard $(CSRC)/*.cu $(CSRC)/*.cuh $(CSRC)/*.hpp) include/daccord_b200.h
-HOSTDEPS := $(wildcard $(CSRC)/host/*.hpp $(CSRC)/host/*.cpp) $(CSRC)/profile_core.cuh $(CSRC)/inqual_core.cuh $(CSRC)/exqual_core.cuh include/daccord_b200.h
+HOSTDEPS := $(wildcard $(CSRC)/host/*.hpp $(CSRC)/host/*.cpp) $(CSRC)/profile_core.cuh $(CSRC)/inqual_core.cuh $(CSRC)/exqual_core.cuh $(CSRC)/proper_core.cuh include/daccord_b200.h
 
-all: $(B)/libdaccord_b200.so $(B)/libdaccord_host.so $(B)/daccord $(B)/computeintrinsicqv $(B)/computeextrinsicqv oracle
+all: $(B)/libdaccord_b200.so $(B)/libdaccord_host.so $(B)/daccord $(B)/computeintrinsicqv $(B)/computeextrinsicqv $(B)/lasfilteralignments oracle
 
 $(B)/libdaccord_b200.so: $(CUDEPS)
 	@mkdir -p $(B)
@@ -29,6 +29,9 @@ $(B)/computeintrinsicqv: $(HOSTDEPS) $(B)/libdaccord_b200.so
 
 $(B)/computeextrinsicqv: $(HOSTDEPS) $(B)/libdaccord_b200.so
 	$(CXX) $(CXXFLAGS) -o $@ $(CSRC)/host/computeextrinsicqv.cpp -L$(B) -ldaccord_b200 -Wl,-rpath,'$$ORIGIN'
+
+$(B)/lasfilteralignments: $(HOSTDEPS) $(B)/libdaccord_b200.so
+	$(CXX) $(CXXFLAGS) -o $@ $(CSRC)/host/lasfilteralignments.cpp -L$(B) -ldaccord_b200 -Wl,-rpath,'$$ORIGIN'
 
 oracle:
 	$(MAKE) -s -C oracle

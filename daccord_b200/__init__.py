@@ -21,6 +21,7 @@ FRAGMENT_DT = np.dtype([("aread", "<u4"), ("from", "<u4"), ("to", "<u4"), ("rese
 PROF_SKIPPED, PROF_REPEAT, PROF_NO_CONSENSUS, PROF_OK = 0, 1, 2, 3
 CONS_STRIDE, OPS_STRIDE = 64, 128
 WIN_SKIPPED, WIN_OK, WIN_FAILED = 0, 1, 2
+PROPER_LEFT, PROPER_RIGHT = 1, 2
 
 
 class Params(C.Structure):
@@ -173,6 +174,31 @@ class Engine:
         ms, rt, hf = C.c_float(0), C.c_uint64(0), C.c_uint64(0)
         self._ck(self.lib.dcu_last_exqual_stats(self.ctx, C.byref(ms), C.byref(rt), C.byref(hf)))
         return {"kernel_ms": ms.value, "retried": rt.value, "host_fragments": hf.value}
+
+    def set_inqual(self, track, offsets, read_len, tspace):
+        """upload the whole-DB inqual track for proper (dcu_set_inqual): track = the tile bytes in read order, offsets = reads + 1 offsets into
+        it (the .anno's), read_len = every read's length; read r must have ceil(read_len[r] / tspace) bytes"""
+        track = np.ascontiguousarray(track, np.uint8)
+        offsets = np.ascontiguousarray(offsets, np.uint64)
+        read_len = np.ascontiguousarray(read_len, np.uint32)
+        if len(offsets) != len(read_len) + 1:
+            raise DcuError("set_inqual: %d offsets for %d reads" % (len(offsets), len(read_len)))
+        self._ck(self.lib.dcu_set_inqual(self.ctx, _p(track), C.c_uint64(len(track)), _p(offsets), _p(read_len), C.c_uint64(len(read_len)), C.c_int32(tspace)))
+
+    def proper(self, ovl, termval):
+        """proper alignment ends on the GPU (dcu_proper) against the track of set_inqual: ovl as daccord_b200.host.OVERLAP_DT; returns one uint8 per
+        overlap, PROPER_LEFT | PROPER_RIGHT when both ends terminate (lasfilteralignments keeps those)"""
+        from .host import term_byte
+        ovl = np.ascontiguousarray(ovl)
+        out = np.zeros(max(len(ovl), 1), np.uint8)
+        self._ck(self.lib.dcu_proper(self.ctx, _p(ovl), C.c_uint64(len(ovl)), C.c_uint32(term_byte(termval)), _p(out)))
+        return out[:len(ovl)]
+
+    def proper_stats(self):
+        """the last proper call: kernel time in ms (CUDA events, dcu_last_proper_stats)"""
+        ms = C.c_float(0)
+        self._ck(self.lib.dcu_last_proper_stats(self.ctx, C.byref(ms)))
+        return {"kernel_ms": ms.value}
 
     def get_windows(self, with_slices=False):
         win = np.zeros(self.nwin, WINDOW_DT)

@@ -43,7 +43,8 @@ def build(force=False, verbose=False):
     host_deps = [os.path.join(csrc, "host", f) for f in os.listdir(os.path.join(csrc, "host"))] + [os.path.join(ROOT, "include", "daccord_b200.h"),
                                                                                                os.path.join(csrc, "profile_core.cuh"),
                                                                                                os.path.join(csrc, "inqual_core.cuh"),
-                                                                                               os.path.join(csrc, "exqual_core.cuh")]
+                                                                                               os.path.join(csrc, "exqual_core.cuh"),
+                                                                                               os.path.join(csrc, "proper_core.cuh")]
     if force or _newer(HOST_LIB, host_deps):
         subprocess.check_call(["/usr/bin/g++", "-O3", "-g", "-std=c++17", "-march=x86-64-v2", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared",
                                "-o", HOST_LIB, host_src])
@@ -59,6 +60,10 @@ def build(force=False, verbose=False):
     if force or _newer(xqv, host_deps + [LIB]):
         subprocess.check_call(["/usr/bin/g++", "-O3", "-g", "-std=c++17", "-march=x86-64-v2", "-ffp-contract=off", "-fopenmp", "-pthread", "-o", xqv,
                                os.path.join(csrc, "host", "computeextrinsicqv.cpp"), "-L" + BUILD, "-ldaccord_b200", "-Wl,-rpath,$ORIGIN"])
+    lfa = os.path.join(BUILD, "lasfilteralignments")
+    if force or _newer(lfa, host_deps + [LIB]):
+        subprocess.check_call(["/usr/bin/g++", "-O3", "-g", "-std=c++17", "-march=x86-64-v2", "-ffp-contract=off", "-fopenmp", "-pthread", "-o", lfa,
+                               os.path.join(csrc, "host", "lasfilteralignments.cpp"), "-L" + BUILD, "-ldaccord_b200", "-Wl,-rpath,$ORIGIN"])
     return LIB
 
 

@@ -45,12 +45,15 @@ __device__ unsigned long long g_stage_clk[CLK_N];
 #include "profile_load.cuh"           // prof_load: a profile window's slices decoded into its scratch
 #include "inqual_core.cuh"            // namespace dinq: the intrinsic quality track (dcu_inqual)
 #include "exqual_core.cuh"            // namespace dxq: the extrinsic quality track (dcu_exqual)
+#include "proper_core.cuh"            // namespace dprop: proper alignment ends against the inqual track (dcu_proper)
 #include "../../include/daccord_b200.h"
 
 static_assert(sizeof(dcu::Slice) == sizeof(dcu_slice) && sizeof(dcu::Window) == sizeof(dcu_window) && sizeof(dcu::Result) == sizeof(dcu_result), "ABI structs");
 static_assert(sizeof(dvote::Win) == sizeof(dcu_window) && sizeof(dvote::Res) == sizeof(dcu_result), "ABI structs (vote)");
 static_assert(sizeof(dinq::Ovl) == sizeof(dcu_overlap) && offsetof(dinq::Ovl, tlen) == offsetof(dcu_overlap, tlen) && offsetof(dinq::Ovl, trace_off) == offsetof(dcu_overlap, trace_off),
               "ABI structs (inqual)");
+static_assert(sizeof(dprop::Ovl) == sizeof(dcu_overlap) && offsetof(dprop::Ovl, flags) == offsetof(dcu_overlap, flags) && offsetof(dprop::Ovl, bread) == offsetof(dcu_overlap, bread) &&
+              (int)dprop::PROPER_LEFT == (int)DCU_PROPER_LEFT && (int)dprop::PROPER_RIGHT == (int)DCU_PROPER_RIGHT, "ABI structs (proper)");
 static_assert(sizeof(dxq::Frag) == sizeof(dcu_fragment) && offsetof(dxq::Frag, off) == offsetof(dcu_fragment, off), "ABI structs (exqual)");
 
 namespace {
@@ -528,6 +531,16 @@ __global__ void xq_min_k(const dxq::Read* reads, const dxq::Frag* fr, const uint
   }
 }
 
+// ---- proper alignment ends (proper_core.cuh): one thread per overlap, both reads' tile bytes from the resident whole-DB track
+constexpr int PROP_TPB = 256;
+__global__ void __launch_bounds__(PROP_TPB) prop_k(const dprop::Ovl* ov, uint64_t n, const uint8_t* track, const uint64_t* toff, const uint32_t* rlen,
+                                                   int32_t tspace, uint32_t term, uint8_t* out) {
+  const uint64_t i = (uint64_t)blockIdx.x * PROP_TPB + threadIdx.x;
+  if (i >= n) return;
+  const dprop::Ovl o = ov[i];
+  out[i] = (uint8_t)dprop::flags(o, rlen[o.aread], rlen[o.bread], track + toff[o.aread], track + toff[o.bread], tspace, term);
+}
+
 // ---- pile vote (vote_core.cuh): per window the offset table, per A position the column votes (count pass, then fill pass)
 __global__ void vote_k0(const dvote::Res* res, const uint8_t* ops, uint64_t nwin, dvote::Params P, uint16_t* ent, int* err) {
   uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -635,6 +648,10 @@ struct dcu_ctx {
   DevBuf<dxq::Frag> dxfrag; DevBuf<uint8_t> dxcodes, dxscratch, dxout, dxstatus; DevBuf<uint64_t> dxboff, dxfout; DevBuf<uint32_t> dxrlen, dxorder, dxkband;
   DevBuf<dxq::Read> dxreads; DevBuf<unsigned int> dxticket;
   float xq_ms = 0.f; uint64_t xq_retried = 0, xq_host = 0;
+  // proper alignment ends (dcu_set_inqual / dcu_proper): the resident whole-DB track, its offsets and read lengths (and a host copy of the
+  // lengths for the batch check), the batch's overlaps and flags, the last kernel time
+  DevBuf<uint8_t> dptrack, dpflags; DevBuf<uint64_t> dptoff; DevBuf<uint32_t> dpqlen; DevBuf<dprop::Ovl> dpovl;
+  std::vector<uint32_t> pq_len; int32_t pq_tspace = 0; bool pq_set = false; float pq_ms = 0.f;
   std::string err;
 };
 
@@ -725,6 +742,7 @@ void dcu_destroy(dcu_ctx* ctx) {
   ctx->dqovl.release(); ctx->dqtrace.release(); ctx->dqreads.release(); ctx->dqitems.release(); ctx->dqout.release();
   ctx->dxfrag.release(); ctx->dxcodes.release(); ctx->dxscratch.release(); ctx->dxout.release(); ctx->dxstatus.release(); ctx->dxboff.release();
   ctx->dxfout.release(); ctx->dxrlen.release(); ctx->dxorder.release(); ctx->dxkband.release(); ctx->dxreads.release(); ctx->dxticket.release();
+  ctx->dptrack.release(); ctx->dpflags.release(); ctx->dptoff.release(); ctx->dpqlen.release(); ctx->dpovl.release();
   if (ctx->hwin) cudaFreeHost(ctx->hwin);
   if (ctx->ev0) cudaEventDestroy(ctx->ev0);
   if (ctx->ev1) cudaEventDestroy(ctx->ev1);
@@ -1084,6 +1102,64 @@ int dcu_last_inqual_stats(dcu_ctx* ctx, float* kernel_ms, uint32_t* bins, uint32
   if (kernel_ms) *kernel_ms = ctx->inq_ms;
   if (bins) *bins = ctx->inq_nb;
   if (tiles_per_block) *tiles_per_block = ctx->inq_ch;
+  return DCU_OK;
+}
+
+// the whole-DB inqual track for dcu_proper: checked against the read lengths on the host, then resident on the device
+int dcu_set_inqual(dcu_ctx* ctx, const uint8_t* bytes, uint64_t nbytes, const uint64_t* read_toff, const uint32_t* read_len, uint64_t nreads,
+                   int32_t tspace) {
+  if (!ctx || (!bytes && nbytes) || !read_toff || (!read_len && nreads)) return DCU_ERR_PARAM;
+  ctx->pq_set = false;
+  if (tspace < 1) { ctx->err = "tspace must be positive"; return DCU_ERR_PARAM; }
+  if (nreads >= 0x7FFFFFFFull) { ctx->err = "more reads than a .las can name"; return DCU_ERR_PARAM; }
+  for (uint64_t r = 0; r < nreads; ++r) {
+    if (read_toff[r + 1] < read_toff[r] || read_toff[r + 1] > nbytes) { ctx->err = "track offsets decrease or pass the track's bytes at read " + std::to_string(r); return DCU_ERR_PARAM; }
+    const uint64_t want = ((uint64_t)read_len[r] + (uint64_t)tspace - 1) / (uint64_t)tspace;
+    if (read_toff[r + 1] - read_toff[r] != want) {
+      ctx->err = "read " + std::to_string(r) + " has " + std::to_string(read_toff[r + 1] - read_toff[r]) + " track bytes, ceil(" + std::to_string(read_len[r]) + " / " +
+                 std::to_string(tspace) + ") = " + std::to_string(want) + " expected";
+      return DCU_ERR_PARAM;
+    }
+  }
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  CK(ctx->dptrack.ensure(nbytes + 1)); CK(ctx->dptoff.ensure(nreads + 1)); CK(ctx->dpqlen.ensure(nreads + 1));
+  if (nbytes) CK(cudaMemcpyAsync(ctx->dptrack.p, bytes, nbytes, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(ctx->dptoff.p, read_toff, (nreads + 1) * 8, cudaMemcpyHostToDevice, st));
+  if (nreads) CK(cudaMemcpyAsync(ctx->dpqlen.p, read_len, nreads * 4, cudaMemcpyHostToDevice, st));
+  CK(cudaStreamSynchronize(st));
+  ctx->pq_len.assign(read_len, read_len + nreads); ctx->pq_tspace = tspace; ctx->pq_set = true;
+  return DCU_OK;
+}
+
+// one flag byte per overlap: the batch checked on the host (dprop::check), then one thread per overlap (prop_k).  The resident batch is not touched.
+int dcu_proper(dcu_ctx* ctx, const dcu_overlap* ovl, uint64_t novl, uint32_t term_byte, uint8_t* out_flags) {
+  if (!ctx || (!ovl && novl) || (!out_flags && novl)) return DCU_ERR_PARAM;
+  if (!ctx->pq_set) { ctx->err = "dcu_proper before dcu_set_inqual"; return DCU_ERR_STATE; }
+  if (term_byte > 256) { ctx->err = "term_byte above 256"; return DCU_ERR_PARAM; }
+  const dprop::Ovl* ov = reinterpret_cast<const dprop::Ovl*>(ovl);
+  uint64_t bad = 0;
+  if (const char* e = dprop::check(ov, novl, ctx->pq_len.data(), ctx->pq_len.size(), &bad)) { ctx->err = std::string(e) + " (overlap " + std::to_string(bad) + ")"; return DCU_ERR_PARAM; }
+  ctx->pq_ms = 0.f;
+  if (!novl) return DCU_OK;
+  if ((novl + PROP_TPB - 1) / PROP_TPB >= 0x7FFFFFFFull) { ctx->err = "batch too large"; return DCU_ERR_UNSUPPORTED; }
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  CK(ctx->dpovl.ensure(novl)); CK(ctx->dpflags.ensure(novl));
+  CK(cudaMemcpyAsync(ctx->dpovl.p, ov, novl * sizeof(dprop::Ovl), cudaMemcpyHostToDevice, st));
+  CK(cudaEventRecord(ctx->ev0, st));
+  prop_k<<<(unsigned)((novl + PROP_TPB - 1) / PROP_TPB), PROP_TPB, 0, st>>>(ctx->dpovl.p, novl, ctx->dptrack.p, ctx->dptoff.p, ctx->dpqlen.p, ctx->pq_tspace, term_byte,
+                                                                          ctx->dpflags.p);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(ctx->ev1, st));
+  CK(cudaMemcpyAsync(out_flags, ctx->dpflags.p, novl, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  CK(cudaEventElapsedTime(&ctx->pq_ms, ctx->ev0, ctx->ev1));
+  return DCU_OK;
+}
+int dcu_last_proper_stats(dcu_ctx* ctx, float* kernel_ms) {
+  if (!ctx) return DCU_ERR_PARAM;
+  if (kernel_ms) *kernel_ms = ctx->pq_ms;
   return DCU_OK;
 }
 

@@ -18,6 +18,7 @@
 #include "vote.hpp"
 #include "eprof.hpp"
 #include "truth.hpp"
+#include "../proper_core.cuh"
 
 using namespace dhost;
 
@@ -366,5 +367,18 @@ uint64_t dh_banded_distance(const char* a, uint64_t la, const char* b, uint64_t 
 // the four counts of an error profile file (binary as the reference writes it, or this repository's earlier text form)
 int dh_read_eprof(const char* fn, uint64_t* out4) { return read_eprof(fn, out4) ? 0 : 1; }
 void dh_free(void* p) { free(p); }
+// the host build of dcu_proper (proper_core.cuh, what lasfilteralignments runs without a device): one flag byte per overlap (dcu_overlap form)
+// against the track bytes[read_toff[r] ..) of reads with lengths read_len[0, nreads); term_byte as dprop::term_byte(termval).  The track's
+// shape is the caller's to check (dcu_set_inqual's rule); 1 and *bad = the overlap when one lies outside its reads or the reads.
+int dh_proper(const dcu_overlap* ovl, uint64_t novl, const uint8_t* bytes, const uint64_t* read_toff, const uint32_t* read_len, uint64_t nreads, int32_t tspace,
+              uint32_t term_byte, uint8_t* out_flags, uint64_t* bad) {
+  const dprop::Ovl* ov = reinterpret_cast<const dprop::Ovl*>(ovl);
+  if (tspace < 1 || dprop::check(ov, novl, read_len, nreads, bad)) return 1;
+#pragma omp parallel for schedule(static)
+  for (int64_t i = 0; i < (int64_t)novl; ++i)
+    out_flags[i] = (uint8_t)dprop::flags(ov[i], read_len[ov[i].aread], read_len[ov[i].bread], bytes + read_toff[ov[i].aread], bytes + read_toff[ov[i].bread], tspace, term_byte);
+  return 0;
+}
+uint32_t dh_term_byte(double termval) { return dprop::term_byte(termval); }
 
 }  // extern "C"

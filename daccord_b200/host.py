@@ -25,6 +25,8 @@ def lib():
             getattr(L, f).restype = C.c_uint64
         L.dh_data_error.restype = C.c_char_p
         L.dh_data_readlen.restype = C.c_uint32
+        L.dh_term_byte.restype = C.c_uint32
+        L.dh_term_byte.argtypes = [C.c_double]
         _lib = L
     return _lib
 
@@ -243,6 +245,29 @@ def profile_counts(records):
     out = {k: int(v) for k, v in zip(keys, a)}
     out["eavg"], out["edif"] = float(d[0]), float(d[1])
     return out
+
+
+def term_byte(termval):
+    """the byte from which a tile of the inqual track is bad for lasfilteralignments -e termval: ceil(termval * 255) clamped to [0, 256]
+    (proper_core.cuh dprop::term_byte)"""
+    return int(lib().dh_term_byte(float(termval)))
+
+
+def proper_flags(ovl, track, offsets, read_len, tspace, termval):
+    """the host build of Engine.proper (proper_core.cuh, lasfilteralignments' host path): one uint8 per overlap (OVERLAP_DT), bit 1 = the left
+    end terminates, bit 2 = the right end does, against the whole-DB track bytes `track` with per-read offsets `offsets` (reads + 1)"""
+    ovl = np.ascontiguousarray(ovl, OVERLAP_DT)
+    track = np.ascontiguousarray(track, np.uint8)
+    offsets = np.ascontiguousarray(offsets, np.uint64)
+    read_len = np.ascontiguousarray(read_len, np.uint32)
+    assert len(offsets) == len(read_len) + 1
+    out = np.zeros(max(len(ovl), 1), np.uint8)
+    bad = C.c_uint64(0)
+    if lib().dh_proper(ovl.ctypes.data_as(C.c_void_p), C.c_uint64(len(ovl)), track.ctypes.data_as(C.c_void_p), offsets.ctypes.data_as(C.c_void_p),
+                       read_len.ctypes.data_as(C.c_void_p), C.c_uint64(len(read_len)), C.c_int32(tspace), C.c_uint32(term_byte(termval)),
+                       out.ctypes.data_as(C.c_void_p), C.byref(bad)):
+        raise DcuError("proper_flags: overlap %d lies outside its reads (or tspace < 1)" % bad.value)
+    return out[:len(ovl)]
 
 
 def format_segments(seg, chars, counter=0):

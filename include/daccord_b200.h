@@ -198,6 +198,24 @@ int dcu_exqual(dcu_ctx* ctx, const dcu_fragment* frag, uint64_t nfrag, const uin
 /* the last dcu_exqual: its kernels' time (CUDA events), fragments rerun with twice the first band, fragments finished on the host (their band
  * did not fit the device capacities, or their score exceeded twice the first band) */
 int dcu_last_exqual_stats(dcu_ctx* ctx, float* kernel_ms, uint64_t* retried, uint64_t* host_fragments);
+/* ---- proper alignment ends on the GPU (lasfilteralignments, reference src/lasfilteralignments.cpp) ------------------------------
+ * dcu_set_inqual uploads the whole-DB `inqual` track once: read r's tile bytes are bytes[read_toff[r] .. read_toff[r + 1]) (read_toff holds
+ * nreads + 1 offsets, read_toff[nreads] <= nbytes), one per tile of tspace bases of a read of read_len[r] bases.  DCU_ERR_PARAM when a read
+ * does not have ceil(read_len[r] / tspace) bytes, the offsets decrease or pass nbytes, or tspace < 1.  A later call replaces the track.
+ * dcu_proper writes one flag byte per overlap (dcu_overlap, the dcu_pile form; only the coordinates, flags, aread and bread are read):
+ * DCU_PROPER_LEFT when the left end terminates (abpos == 0, bbpos == 0, or the A tile of base abpos - 1 or the B tile of oriented base
+ * bbpos - 1 is bad), DCU_PROPER_RIGHT when the right end does (aepos == alen, bepos == blen, or the A tile of base aepos or the B tile of
+ * oriented base bepos is bad).  A tile is bad when its byte is >= term_byte (0..256; lasfilteralignments passes ceil(termval * 255)).  B
+ * coordinates are oriented: for flags & 1, oriented base p is forward base blen - 1 - p.  A record is proper, and kept, with both bits
+ * (INTEGRATION.md §3d).  One thread per overlap; neither call touches the resident batch.
+ * DCU_ERR_STATE without dcu_set_inqual; DCU_ERR_PARAM (dcu_last_error says why) for term_byte > 256, a read outside the track's reads, or
+ * coordinates outside 0 <= abpos <= aepos <= alen, 0 <= bbpos <= bepos <= blen. */
+enum { DCU_PROPER_LEFT = 1, DCU_PROPER_RIGHT = 2 };
+int dcu_set_inqual(dcu_ctx* ctx, const uint8_t* bytes, uint64_t nbytes, const uint64_t* read_toff, const uint32_t* read_len, uint64_t nreads,
+                   int32_t tspace);
+int dcu_proper(dcu_ctx* ctx, const dcu_overlap* ovl, uint64_t novl, uint32_t term_byte, uint8_t* out_flags);
+/* the last dcu_proper: its kernel's time (CUDA events) */
+int dcu_last_proper_stats(dcu_ctx* ctx, float* kernel_ms);
 /* statistics of the last launch: kernels launched, windows that needed the large-workspace pass */
 int dcu_last_stats(dcu_ctx* ctx, uint64_t* launches, uint64_t* hard_windows);
 /* more statistics of the last launch: windows the first pass handed to the plain HBM passes, windows beyond every capacity
